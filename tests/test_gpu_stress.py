@@ -204,3 +204,40 @@ def test_one_service_of_120k_spans_equals_oracle():
     assert np.array_equal(out["counters"][:, :2], ref["counters"][:, :2])
     truth = synth.truth_assign([blk])
     assert (out["assign"] == truth).mean() > 0.99
+
+
+def _engine_vs_profiler(eng, fn, trace):
+    """(launch_count() delta, kernels of the library the CUDA profiler recorded) around fn()."""
+    import json
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    l0 = eng.launch_count()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    prof.export_chrome_trace(str(trace))
+    with open(trace) as f:
+        events = json.load(f)["traceEvents"]
+    seen = sum(1 for ev in events if ev.get("cat") == "kernel" and "tw::k_" in ev.get("name", ""))
+    return eng.launch_count() - l0, seen
+
+
+def test_launch_count_matches_profiler(engine, tmp_path):
+    """launch_count() counts the kernels the engine issues, conditional launches included: a whole
+    solve step, the global-memory sort of lists longer than 16 384 spans, accuracy without trace ids."""
+    import torch
+    from traceweaver_b200 import synth, truth
+    from traceweaver_b200.batch import build_batch_from_blocks
+    from traceweaver_b200.predictor import solve_bound
+    engine.bind(build_batch_from_blocks(synth.hotel_stream(6, 200, seed=7)))
+    counted, seen = _engine_vs_profiler(engine, lambda: solve_bound(engine), tmp_path / "solve.json")
+    assert seen > 0 and counted == seen
+    hb = build_batch_from_blocks([synth.make_block("hotel_frontend", 1, 20_000, 100.0, seed=3)])
+    engine.bind(hb)
+    counted, seen = _engine_vs_profiler(engine, engine.prepare, tmp_path / "prepare.json")
+    assert counted == seen == 4                              # prev index, sort, long-list sort, tile windows
+    tl = truth.TraceLists.from_host_batch(hb, None, 0)
+    z = torch.zeros(int(hb.prob_tuple_off[-1]), dtype=torch.int32, device=engine.device)
+    counted, seen = _engine_vs_profiler(engine, lambda: truth.accuracy(engine, tl, z, z), tmp_path / "accuracy.json")
+    assert counted == seen == 2                              # no trace ids: no per-trace reduction

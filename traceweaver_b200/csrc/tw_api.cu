@@ -5,7 +5,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <map>
+#include <memory>
 #include <random>
 #include <string>
 #include <vector>
@@ -29,8 +29,35 @@ static int fail(int code, const char* fmt, const char* a = "", const char* b2 = 
     if (_e != cudaSuccess) return fail(TW_ERR_CUDA, "%s: %s", #expr, cudaGetErrorString(_e)); \
   } while (0)
 
+// Device scratch owned by the engine, grow-only: re-binding a batch of similar size allocates nothing.
+template <class T>
+struct DevBuf {
+  T* p = nullptr;
+  size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
+  // room for `count` elements (1 if 0), with 1/8 headroom when it has to grow.  A reallocation loses
+  // the contents: `valid`, the flag of a cache kept in this buffer, is cleared then.
+  cudaError_t reserve(size_t count, bool* valid = nullptr) {
+    const size_t need = (count ? count : 1) * sizeof(T);
+    if (bytes >= need) return cudaSuccess;
+    if (valid) *valid = false;
+    if (p) cudaFree(p);
+    p = nullptr;
+    bytes = 0;
+    const size_t cap = need + need / 8;
+    cudaError_t e = cudaMalloc((void**)&p, cap);
+    if (e != cudaSuccess) return e;
+    bytes = cap;
+    return cudaSuccess;
+  }
+};
+
 struct tw_engine {
   int device = 0;
+  int n_sm = 0;
   bool bound = false;
   tw_batch dev{};
   int64_t launches = 0;
@@ -39,90 +66,65 @@ struct tw_engine {
   std::vector<int32_t> prob_ep_off;
   int max_seg = 0;
   int64_t dev_n_tuple = 0;
-  // device scratch (owned, grow-only: re-binding a batch of similar size allocates nothing)
-  struct Slot { void* p = nullptr; size_t bytes = 0; };
-  std::map<void*, Slot> slots;
-  int32_t* prev_idx = nullptr;
-  int32_t* score_tiles = nullptr;    // [2*n]: prob, start; grouped by the problem's E (class_off)
-  int32_t* tile_win = nullptr;       // [n][2*TW_MAX_E] candidate slice per ep (k_tile_meta)
-  int32_t* wide_tiles = nullptr;     // [4*n]: prob, start, scoring-tile index, length
+  // device status word: allocated and zeroed with the engine, sticky across re-binds (a caller that
+  // pipelines several batches through one engine reads it once at the end), cleared by tw_engine_status only
+  DevBuf<int> err_flag;
+  DevBuf<int32_t> prev_idx;
+  DevBuf<int32_t> score_tiles;       // [2*n]: prob, start; grouped by the problem's E (class_off)
+  DevBuf<int32_t> tile_win;          // [n][2*TW_MAX_E] candidate slice per ep (k_tile_meta)
+  DevBuf<int32_t> wide_tiles;        // [4*n]: prob, start, scoring-tile index, length
   int n_tiles = 0, n_wide = 0;
   int class_off[TW_MAX_E + 1] = {0};
-  uint8_t* tile_overflow = nullptr;
+  DevBuf<uint8_t> tile_overflow;
   bool windows_valid = false;        // cut / maps / overflow flags of this batch have been produced
-  int32_t* own_used_lo = nullptr;    // candidate maps when the caller does not ask for them
-  uint32_t* own_used_bits = nullptr;
-  uint8_t* own_used_wide = nullptr;
-  uint32_t* taken = nullptr;
+  DevBuf<int32_t> own_used_lo;       // candidate maps when the caller does not ask for them
+  DevBuf<uint32_t> own_used_bits;
+  DevBuf<uint8_t> own_used_wide;
+  DevBuf<uint32_t> taken;
   size_t taken_words = 0;
-  double* fp64_sink = nullptr;       // tw_measure_fp64_peak
+  DevBuf<double> fp64_sink;          // tw_measure_fp64_peak
   // ground truth / order / accuracy scratch (tw_truth.cu)
-  int32_t* truth_tab = nullptr;
-  int64_t* truth_tab_off = nullptr;
-  int32_t* in_prob = nullptr;
-  int* order_missing = nullptr;
-  uint8_t* acc_flags = nullptr;
-  unsigned long long* acc_first = nullptr;
+  DevBuf<int32_t> truth_tab;
+  DevBuf<int64_t> truth_tab_off;
+  DevBuf<int32_t> in_prob;
+  DevBuf<int> order_missing;
+  DevBuf<uint8_t> acc_flags;
+  DevBuf<unsigned long long> acc_first;
   // skip / cache mode scratch (tw_skip_solve)
-  uint32_t* skip_sets = nullptr;
-  int64_t* skip_set_off = nullptr;
-  uint32_t* skip_taken = nullptr;
-  int32_t* skip_win = nullptr;
-  int* err_flag = nullptr;
-  int32_t* unit_prob = nullptr;      // stitch units (k_stitch_units)
-  int32_t* unit_lo = nullptr;
-  int32_t* unit_hi = nullptr;
-  int* unit_count = nullptr;
+  DevBuf<uint32_t> skip_sets;
+  DevBuf<int64_t> skip_set_off;
+  DevBuf<uint32_t> skip_taken;
+  DevBuf<int32_t> skip_win;
+  DevBuf<int32_t> unit_prob;         // stitch units (k_stitch_units)
+  DevBuf<int32_t> unit_lo;
+  DevBuf<int32_t> unit_hi;
+  DevBuf<int> unit_count;
   int max_units = 0;
-  int32_t* long_seg = nullptr;       // lists longer than kSortSmemCap (sorted in global memory)
+  DevBuf<int32_t> long_seg;          // lists longer than kSortSmemCap (sorted in global memory)
   int n_long = 0;
-  int64_t* long_scratch = nullptr;
+  DevBuf<int64_t> long_scratch;
   int64_t slab_len = 1;
-  int64_t* in_end_sorted = nullptr;
-  int64_t* out_end_sorted = nullptr;
-  int32_t* batch_prob = nullptr;
-  int32_t* batch_idx = nullptr;
+  DevBuf<int64_t> in_end_sorted;
+  DevBuf<int64_t> out_end_sorted;
+  DevBuf<int32_t> batch_prob;
+  DevBuf<int32_t> batch_idx;
   int n_batches_total = 0;
-  int32_t* term_ep = nullptr;
-  int32_t* ep_prob = nullptr;
+  DevBuf<int32_t> term_ep;
+  DevBuf<int32_t> ep_prob;
   long long node_limit = 2000000LL;   // exact MWIS search nodes per window before TW_ERR_MWIS_LIMIT
   // refit scratch (allocated on first tw_gmm_refit after bind)
   static constexpr int kStreamLen = 16384;
-  int32_t* gmm_max_n = nullptr;
-  double* gmm_mean_var = nullptr;
-  uint32_t* gmm_skip = nullptr;
-  double* gmm_bic = nullptr;
-  double* gmm_cen = nullptr;      // k-means centres handed from the seeding to the Lloyd to the EM kernels
+  DevBuf<int32_t> gmm_max_n;
+  DevBuf<double> gmm_mean_var;
+  DevBuf<uint32_t> gmm_skip;
+  DevBuf<double> gmm_bic;
+  DevBuf<double> gmm_cen;         // k-means centres handed from the seeding to the Lloyd to the EM kernels
   GmmFork gmm_fork;               // side streams of the five per-K fit chains
-  double* gmm_stream = nullptr;
-  double* gmm_stream100 = nullptr;
+  DevBuf<double> gmm_stream;
+  DevBuf<double> gmm_stream100;
   uint32_t gmm_seed = 0;
-  bool gmm_seed_valid = false;
-
+  bool gmm_seed_valid = false;    // gmm_stream holds the draws of gmm_seed
   bool gmm_stream100_valid = false;
-  void release() {
-    for (auto& kv : slots) cudaFree(kv.second.p);
-    slots.clear();
-    bound = false;
-    gmm_seed_valid = false;
-    gmm_stream100_valid = false;
-  }
-  template <class T>
-  cudaError_t alloc(T** out, size_t count) {
-    size_t need = (count ? count : 1) * sizeof(T);
-    Slot& sl = slots[(void*)out];
-    if (sl.bytes < need) {
-      if (sl.p) cudaFree(sl.p);
-      sl.p = nullptr;
-      sl.bytes = 0;
-      size_t cap = need + need / 8;
-      cudaError_t e = cudaMalloc(&sl.p, cap);
-      if (e != cudaSuccess) return e;
-      sl.bytes = cap;
-    }
-    *out = (T*)sl.p;
-    return cudaSuccess;
-  }
 };
 
 extern "C" {
@@ -147,70 +149,74 @@ int tw_engine_create(int device, tw_engine** out) {
   if (prop.major != 9 || prop.minor != 0)
     return fail(TW_ERR_NO_DEVICE, "tw_engine_create: built for sm_90a (H100), found %s", prop.name);
   CU(cudaSetDevice(device));
-  tw_engine* e = new tw_engine;
+  CU(setup_score3());
+  CU(setup_score());
+  CU(setup_stitch());
+  CU(setup_sort_ends());
+  std::unique_ptr<tw_engine> e(new tw_engine);
   e->device = device;
-  *out = e;
+  e->n_sm = prop.multiProcessorCount;
+  CU(e->err_flag.reserve(1));
+  CU(cudaMemset(e->err_flag.p, 0, sizeof(int)));
+  CU(cudaDeviceSynchronize());   // cudaMemset is asynchronous, and the kernels run on the caller's streams
+  *out = e.release();
   return TW_OK;
 }
 
 int tw_engine_destroy(tw_engine* eng) {
   if (!eng) return TW_OK;
   cudaSetDevice(eng->device);
-  eng->release();
-  if (eng->gmm_fork.ready) {
-    cudaEventDestroy(eng->gmm_fork.fork);
-    for (int q = 0; q < TW_GMM_MAX_COMP; ++q) {
-      cudaEventDestroy(eng->gmm_fork.join[q]);
-      cudaStreamDestroy(eng->gmm_fork.side[q]);
-    }
-  }
   delete eng;
   return TW_OK;
 }
 
-static int validate_host(const tw_batch* h, bool allow_skip);
-int tw_batch_validate_host(const tw_batch* h) { return validate_host(h, false); }
-
-static int validate_host(const tw_batch* h, bool allow_skip) {
-  if (!h || h->n_problems < 1) return fail(TW_ERR_INVALID, "batch: no problems");
-  if (!h->prob_in_off || !h->prob_ep_off || !h->prob_tuple_off || !h->ep_out_off || !h->ep_term_off ||
-      !h->ep_pred_mask || !h->term_src)
-    return fail(TW_ERR_INVALID, "batch: NULL descriptor array");
+// Host-side checks of a batch descriptor.  Every entry point checks the offset tables and the totals.
+// With `terms` (the entry points that solve) also the term lists and the DAG, >= 2 incoming spans per
+// problem and non-empty outgoing lists; outgoing lists must then be as long as the incoming list
+// unless `allow_skip` (tw_skip_solve).
+static int validate_host(const tw_batch* h, const char* who, bool terms, bool allow_skip) {
+  if (!h || h->n_problems < 1) return fail(TW_ERR_INVALID, "%s: no problems", who);
+  if (!h->prob_in_off || !h->prob_ep_off || !h->prob_tuple_off || !h->ep_out_off ||
+      (terms && (!h->ep_term_off || !h->ep_pred_mask || !h->term_src)))
+    return fail(TW_ERR_INVALID, "%s: NULL descriptor array", who);
   const int P = h->n_problems;
   if (h->prob_in_off[0] != 0 || h->prob_ep_off[0] != 0 || h->prob_tuple_off[0] != 0 || h->ep_out_off[0] != 0 ||
-      h->ep_term_off[0] != 0)
-    return fail(TW_ERR_INVALID, "batch: offsets must start at 0");
+      (terms && h->ep_term_off[0] != 0))
+    return fail(TW_ERR_INVALID, "%s: offsets must start at 0", who);
   for (int p = 0; p < P; ++p) {
     int E = h->prob_ep_off[p + 1] - h->prob_ep_off[p];
     int64_t n = h->prob_in_off[p + 1] - h->prob_in_off[p];
-    if (E < 1 || E > TW_MAX_E) return fail(TW_ERR_INVALID, "batch: E outside [1, TW_MAX_E]");
-    if (n < 2 || n > 0x7fffffff) return fail(TW_ERR_INVALID, "batch: a problem needs >= 2 incoming spans");
+    if (E < 1 || E > TW_MAX_E) return fail(TW_ERR_INVALID, "%s: E outside [1, TW_MAX_E]", who);
+    if (n < (terms ? 2 : 1) || n > 0x7fffffff) return fail(TW_ERR_INVALID, "%s: incoming span count out of range", who);
     if (h->prob_tuple_off[p + 1] - h->prob_tuple_off[p] != n * E)
-      return fail(TW_ERR_INVALID, "batch: prob_tuple_off inconsistent");
+      return fail(TW_ERR_INVALID, "%s: prob_tuple_off inconsistent", who);
+    if (!terms) continue;
     int ep0 = h->prob_ep_off[p];
     int nt = h->ep_term_off[ep0 + E] - h->ep_term_off[ep0];
-    if (nt < E || nt > TW_MAX_TERMS) return fail(TW_ERR_INVALID, "batch: term count out of range");
+    if (nt < E || nt > TW_MAX_TERMS) return fail(TW_ERR_INVALID, "%s: term count out of range", who);
     for (int e = 0; e < E; ++e) {
       int64_t no = h->ep_out_off[ep0 + e + 1] - h->ep_out_off[ep0 + e];
       if (no != n && !allow_skip)
-        return fail(TW_ERR_UNSUPPORTED, "batch: n_out != n_in (skip budgets): use tw_skip_solve for this service");
-      if (no < 1) return fail(TW_ERR_INVALID, "batch: an outgoing list is empty");
+        return fail(TW_ERR_UNSUPPORTED, "%s: n_out != n_in (skip budgets): use tw_skip_solve for this service", who);
+      if (no < 1) return fail(TW_ERR_INVALID, "%s: an outgoing list is empty", who);
       uint32_t pm = h->ep_pred_mask[ep0 + e];
-      if (pm >> e) return fail(TW_ERR_INVALID, "batch: predecessor mask must reference earlier eps only");
+      if (pm >> e) return fail(TW_ERR_INVALID, "%s: predecessor mask must reference earlier eps only", who);
       int t0 = h->ep_term_off[ep0 + e], t1 = h->ep_term_off[ep0 + e + 1];
-      if (t1 <= t0 || h->term_src[t1 - 1] != TW_TERM_LAST) return fail(TW_ERR_INVALID, "batch: ep terms must end with LAST");
+      if (t1 <= t0 || h->term_src[t1 - 1] != TW_TERM_LAST) return fail(TW_ERR_INVALID, "%s: ep terms must end with LAST", who);
       for (int t = t0; t < t1 - 1; ++t) {
         int src = h->term_src[t];
-        if (src == TW_TERM_ROOT) { if (pm) return fail(TW_ERR_INVALID, "batch: ROOT term on an ep with in-edges"); }
-        else if (src < 0 || src >= e || !(pm >> src & 1u)) return fail(TW_ERR_INVALID, "batch: edge term without DAG edge");
+        if (src == TW_TERM_ROOT) { if (pm) return fail(TW_ERR_INVALID, "%s: ROOT term on an ep with in-edges", who); }
+        else if (src < 0 || src >= e || !(pm >> src & 1u)) return fail(TW_ERR_INVALID, "%s: edge term without DAG edge", who);
       }
     }
   }
-  if (h->prob_in_off[P] != h->n_in_total || h->ep_out_off[h->prob_ep_off[P]] != h->n_out_total ||
-      h->prob_ep_off[P] != h->n_ep_total || h->ep_term_off[h->n_ep_total] != h->n_term_total)
-    return fail(TW_ERR_INVALID, "batch: totals inconsistent");
+  if (h->prob_in_off[P] != h->n_in_total || h->prob_ep_off[P] != h->n_ep_total ||
+      h->ep_out_off[h->n_ep_total] != h->n_out_total || (terms && h->ep_term_off[h->n_ep_total] != h->n_term_total))
+    return fail(TW_ERR_INVALID, "%s: totals inconsistent", who);
   return TW_OK;
 }
+
+int tw_batch_validate_host(const tw_batch* h) { return validate_host(h, "batch", true, false); }
 
 int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void* stream_) {
   if (!eng || !dev || !h) return fail(TW_ERR_INVALID, "tw_engine_bind: NULL argument");
@@ -267,40 +273,32 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
       for (int t = h->ep_term_off[ep]; t < h->ep_term_off[ep + 1]; ++t) term_ep[t] = ep;
     }
 
-  CU(eng->alloc(&eng->prev_idx, (size_t)h->n_in_total));
-  CU(eng->alloc(&eng->score_tiles, (size_t)eng->n_tiles * 2));
-  CU(eng->alloc(&eng->tile_win, (size_t)eng->n_tiles * 2 * TW_MAX_E));
-  CU(eng->alloc(&eng->wide_tiles, (size_t)eng->n_wide * 4));
-  CU(eng->alloc(&eng->tile_overflow, (size_t)eng->n_tiles));
+  CU(eng->prev_idx.reserve((size_t)h->n_in_total));
+  CU(eng->score_tiles.reserve((size_t)eng->n_tiles * 2));
+  CU(eng->tile_win.reserve((size_t)eng->n_tiles * 2 * TW_MAX_E));
+  CU(eng->wide_tiles.reserve((size_t)eng->n_wide * 4));
+  CU(eng->tile_overflow.reserve((size_t)eng->n_tiles));
   eng->taken_words = (size_t)(h->n_out_total / 32) + (size_t)h->n_ep_total + 2;
-  CU(eng->alloc(&eng->taken, eng->taken_words));
-  {
-    // the device status word is sticky across re-binds (a caller that pipelines several batches
-    // through one engine reads it once at the end): cleared when first allocated and by
-    // tw_engine_status only
-    int* before = eng->err_flag;
-    CU(eng->alloc(&eng->err_flag, 1));
-    if (eng->err_flag != before) CU(cudaMemsetAsync(eng->err_flag, 0, sizeof(int), s));
-  }
-  CU(eng->alloc(&eng->in_end_sorted, (size_t)h->n_in_total));
-  CU(eng->alloc(&eng->out_end_sorted, (size_t)h->n_out_total));
-  CU(eng->alloc(&eng->batch_prob, bprob.size()));
-  CU(eng->alloc(&eng->batch_idx, bidx.size()));
-  CU(eng->alloc(&eng->term_ep, term_ep.size()));
-  CU(eng->alloc(&eng->ep_prob, ep_prob.size()));
+  CU(eng->taken.reserve(eng->taken_words));
+  CU(eng->in_end_sorted.reserve((size_t)h->n_in_total));
+  CU(eng->out_end_sorted.reserve((size_t)h->n_out_total));
+  CU(eng->batch_prob.reserve(bprob.size()));
+  CU(eng->batch_idx.reserve(bidx.size()));
+  CU(eng->term_ep.reserve(term_ep.size()));
+  CU(eng->ep_prob.reserve(ep_prob.size()));
   auto up = [&](void* dst, const std::vector<int32_t>& src) {
     return cudaMemcpyAsync(dst, src.data(), src.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s);
   };
-  CU(up(eng->score_tiles, nt_prob));
-  CU(up(eng->score_tiles + eng->n_tiles, nt_start));
-  CU(up(eng->wide_tiles, wt_prob));
-  CU(up(eng->wide_tiles + eng->n_wide, wt_start));
-  CU(up(eng->wide_tiles + 2 * eng->n_wide, wt_narrow));
-  CU(up(eng->wide_tiles + 3 * eng->n_wide, wt_len));
-  CU(up(eng->batch_prob, bprob));
-  CU(up(eng->batch_idx, bidx));
-  CU(up(eng->term_ep, term_ep));
-  CU(up(eng->ep_prob, ep_prob));
+  CU(up(eng->score_tiles.p, nt_prob));
+  CU(up(eng->score_tiles.p + eng->n_tiles, nt_start));
+  CU(up(eng->wide_tiles.p, wt_prob));
+  CU(up(eng->wide_tiles.p + eng->n_wide, wt_start));
+  CU(up(eng->wide_tiles.p + 2 * eng->n_wide, wt_narrow));
+  CU(up(eng->wide_tiles.p + 3 * eng->n_wide, wt_len));
+  CU(up(eng->batch_prob.p, bprob));
+  CU(up(eng->batch_idx.p, bidx));
+  CU(up(eng->term_ep.p, term_ep));
+  CU(up(eng->ep_prob.p, ep_prob));
   CU(cudaStreamSynchronize(s));   // staging vectors go out of scope
 
   // unit list of the stitch kernel: at most n / kStitchUnitMin + 1 units per service
@@ -309,10 +307,10 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
     for (int p = 0; p < P; ++p) mu += (h->prob_in_off[p + 1] - h->prob_in_off[p]) / kStitchUnitMin + 1;
     if (mu > 0x7fffffff) return fail(TW_ERR_RANGE_LIMIT, "bind: too many stitch units");
     eng->max_units = (int)mu;
-    CU(eng->alloc(&eng->unit_prob, (size_t)mu));
-    CU(eng->alloc(&eng->unit_lo, (size_t)mu));
-    CU(eng->alloc(&eng->unit_hi, (size_t)mu));
-    CU(eng->alloc(&eng->unit_count, 1));
+    CU(eng->unit_prob.reserve((size_t)mu));
+    CU(eng->unit_lo.reserve((size_t)mu));
+    CU(eng->unit_hi.reserve((size_t)mu));
+    CU(eng->unit_count.reserve(1));
   }
   // lists too long for the shared-memory sort of tw_prepare get a slab of global scratch each
   {
@@ -331,10 +329,10 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
     eng->n_long = (int)long_seg.size();
     eng->slab_len = 1;
     while (eng->slab_len < longest) eng->slab_len <<= 1;
-    CU(eng->alloc(&eng->long_seg, long_seg.size()));
-    CU(eng->alloc(&eng->long_scratch, (size_t)eng->n_long * (size_t)eng->slab_len));
+    CU(eng->long_seg.reserve(long_seg.size()));
+    CU(eng->long_scratch.reserve((size_t)eng->n_long * (size_t)eng->slab_len));
     if (eng->n_long) {
-      CU(cudaMemcpyAsync(eng->long_seg, long_seg.data(), long_seg.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+      CU(cudaMemcpyAsync(eng->long_seg.p, long_seg.data(), long_seg.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
       CU(cudaStreamSynchronize(s));
     }
   }
@@ -346,12 +344,11 @@ int tw_prepare(tw_engine* eng, void* stream_) {
   if (!eng || !eng->bound) return fail(TW_ERR_INVALID, "tw_prepare: no batch bound");
   cudaStream_t s = (cudaStream_t)stream_;
   CU(cudaSetDevice(eng->device));
-  CU(launch_prev_index(eng->dev, eng->prev_idx, s));
-  CU(launch_sort_ends(eng->dev, eng->in_end_sorted, eng->out_end_sorted, eng->max_seg, eng->long_seg, eng->n_long,
-                      eng->long_scratch, eng->slab_len, eng->err_flag, s));
-  TileList tl{eng->score_tiles, eng->score_tiles + eng->n_tiles, eng->n_tiles, kS3Tile};
-  CU(launch_tile_meta(eng->dev, tl, eng->tile_win, s));
-  eng->launches += 3;
+  CU(launch_prev_index(eng->dev, eng->prev_idx.p, s, eng->launches));
+  CU(launch_sort_ends(eng->dev, eng->in_end_sorted.p, eng->out_end_sorted.p, eng->max_seg, eng->long_seg.p, eng->n_long,
+                      eng->long_scratch.p, eng->slab_len, eng->err_flag.p, s, eng->launches));
+  TileList tl{eng->score_tiles.p, eng->score_tiles.p + eng->n_tiles, eng->n_tiles, kS3Tile};
+  CU(launch_tile_meta(eng->dev, tl, eng->tile_win.p, s, eng->launches));
   return TW_OK;
 }
 
@@ -359,10 +356,10 @@ int tw_engine_status(tw_engine* eng, void* stream_) {
   if (!eng) return fail(TW_ERR_INVALID, "tw_engine_status: NULL engine");
   cudaStream_t s = (cudaStream_t)stream_;
   int flag = 0;
-  CU(cudaMemcpyAsync(&flag, eng->err_flag, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(&flag, eng->err_flag.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
   if (flag != 0) {
-    CU(cudaMemsetAsync(eng->err_flag, 0, sizeof(int), s));
+    CU(cudaMemsetAsync(eng->err_flag.p, 0, sizeof(int), s));
     return fail(flag, "device-side status %s", flag == TW_ERR_MWIS_LIMIT ? "TW_ERR_MWIS_LIMIT"
                                                : flag == TW_ERR_RANGE_LIMIT ? "TW_ERR_RANGE_LIMIT"
                                                : flag == TW_ERR_REFERENCE_UNDEFINED ? "TW_ERR_REFERENCE_UNDEFINED" : "error");
@@ -381,7 +378,7 @@ int tw_engine_tile_stats(tw_engine* eng, int64_t* n_tiles, int64_t* n_redone, vo
     std::vector<uint8_t> h((size_t)eng->n_tiles);
     *n_redone = 0;
     if (eng->windows_valid) {
-      CU(cudaMemcpyAsync(h.data(), eng->tile_overflow, h.size(), cudaMemcpyDeviceToHost, s));
+      CU(cudaMemcpyAsync(h.data(), eng->tile_overflow.p, h.size(), cudaMemcpyDeviceToHost, s));
       CU(cudaStreamSynchronize(s));
       for (uint8_t f : h) *n_redone += f != 0;
     }
@@ -392,7 +389,7 @@ int tw_engine_tile_stats(tw_engine* eng, int64_t* n_tiles, int64_t* n_redone, vo
 int tw_skip_solve(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const tw_skip_desc* sd, const tw_skip_out* out,
                   void* stream_) {
   if (!eng || !dev || !h || !sd || !out) return fail(TW_ERR_INVALID, "tw_skip_solve: NULL argument");
-  int rc = validate_host(h, true);
+  int rc = validate_host(h, "batch", true, true);
   if (rc) return rc;
   if (!out->pass.assign || !out->pass.mis_rank || !out->pass.n_cand || !out->pass.counters || !out->top2_score ||
       !out->top2_idx || !out->top2_cnt || !out->cut)
@@ -411,26 +408,20 @@ int tw_skip_solve(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const 
       words += (h->ep_out_off[ep + 1] - h->ep_out_off[ep] + 31) / 32;
     set_off[p + 1] = set_off[p] + words;
   }
-  CU(eng->alloc(&eng->skip_sets, (size_t)(3 * set_off[P])));
-  CU(eng->alloc(&eng->skip_set_off, (size_t)P + 1));
-  CU(eng->alloc(&eng->skip_taken, (size_t)(h->n_out_total / 32) + (size_t)h->n_ep_total + 2));
+  CU(eng->skip_sets.reserve((size_t)(3 * set_off[P])));
+  CU(eng->skip_set_off.reserve((size_t)P + 1));
+  CU(eng->skip_taken.reserve((size_t)(h->n_out_total / 32) + (size_t)h->n_ep_total + 2));
   // per (ep, window) prefix + fetch counters: the host does not know prob_cnt_off (device array), so
   // size it by an upper bound the caller's skip_count array must respect: read the last offset
   int64_t cnt_total = 0;
   CU(cudaMemcpyAsync(&cnt_total, sd->prob_cnt_off + P, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
   if (cnt_total < 0) return fail(TW_ERR_INVALID, "tw_skip_solve: prob_cnt_off inconsistent");
-  CU(eng->alloc(&eng->skip_win, (size_t)(2 * cnt_total)));
-  {
-    int* before = eng->err_flag;
-    CU(eng->alloc(&eng->err_flag, 1));
-    if (eng->err_flag != before) CU(cudaMemsetAsync(eng->err_flag, 0, sizeof(int), s));
-  }
-  CU(cudaMemcpyAsync(eng->skip_set_off, set_off.data(), set_off.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
-  CU(launch_skip(*dev, *sd, *out, eng->skip_taken, eng->skip_sets, eng->skip_set_off, eng->skip_win, eng->node_limit,
-                 eng->err_flag, s));
+  CU(eng->skip_win.reserve((size_t)(2 * cnt_total)));
+  CU(cudaMemcpyAsync(eng->skip_set_off.p, set_off.data(), set_off.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  CU(launch_skip(*dev, *sd, *out, eng->skip_taken.p, eng->skip_sets.p, eng->skip_set_off.p, eng->skip_win.p,
+                 eng->node_limit, eng->err_flag.p, s, eng->launches));
   CU(cudaStreamSynchronize(s));    // set_off goes out of scope
-  eng->launches += 1;
   return TW_OK;
 }
 
@@ -439,8 +430,7 @@ int tw_build_dist_samples(tw_engine* eng, int32_t n, const int64_t* start, const
   if (!eng || n < 0 || !start || !end || !label || !key_out || !val_out || E < 1 || E > TW_MAX_E)
     return fail(TW_ERR_INVALID, "tw_build_dist_samples: bad argument");
   CU(cudaSetDevice(eng->device));
-  CU(launch_build_dist(n, start, end, label, E, large_delay, key_out, val_out, (cudaStream_t)stream_));
-  eng->launches += 1;
+  CU(launch_build_dist(n, start, end, label, E, large_delay, key_out, val_out, (cudaStream_t)stream_, eng->launches));
   return TW_OK;
 }
 
@@ -458,19 +448,17 @@ int tw_measure_fp64_peak(tw_engine* eng, double* tflops_out, void* stream_) {
   if (!eng || !tflops_out) return fail(TW_ERR_INVALID, "tw_measure_fp64_peak: NULL argument");
   cudaStream_t s = (cudaStream_t)stream_;
   CU(cudaSetDevice(eng->device));
-  cudaDeviceProp prop;
-  CU(cudaGetDeviceProperties(&prop, eng->device));
-  CU(eng->alloc(&eng->fp64_sink, 1));
-  double* sink = eng->fp64_sink;
-  const int blocks = prop.multiProcessorCount * 8, iters = 1 << 15;
+  CU(eng->fp64_sink.reserve(1));
+  double* sink = eng->fp64_sink.p;
+  const int blocks = eng->n_sm * 8, iters = 1 << 15;
   cudaEvent_t a, b;
   CU(cudaEventCreate(&a));
   CU(cudaEventCreate(&b));
-  CU(launch_fp64_peak(blocks, 1 << 10, sink, s));            // warm-up
+  CU(launch_fp64_peak(blocks, 1 << 10, sink, s, eng->launches));   // warm-up
   double best = 0.0;
   for (int rep = 0; rep < 3; ++rep) {
     CU(cudaEventRecord(a, s));
-    CU(launch_fp64_peak(blocks, iters, sink, s));
+    CU(launch_fp64_peak(blocks, iters, sink, s, eng->launches));
     CU(cudaEventRecord(b, s));
     CU(cudaEventSynchronize(b));
     float ms = 0.f;
@@ -485,26 +473,10 @@ int tw_measure_fp64_peak(tw_engine* eng, double* tflops_out, void* stream_) {
   return TW_OK;
 }
 
-static int offsets_ok(const tw_batch* h, const char* who) {
-  if (!h || h->n_problems < 1 || !h->prob_in_off || !h->prob_ep_off || !h->prob_tuple_off || !h->ep_out_off)
-    return fail(TW_ERR_INVALID, "%s: NULL offset table", who);
-  const int P = h->n_problems;
-  for (int p = 0; p < P; ++p) {
-    const int E = h->prob_ep_off[p + 1] - h->prob_ep_off[p];
-    const int64_t n = h->prob_in_off[p + 1] - h->prob_in_off[p];
-    if (E < 1 || E > TW_MAX_E || n < 1 || h->prob_tuple_off[p + 1] - h->prob_tuple_off[p] != n * E)
-      return fail(TW_ERR_INVALID, "%s: inconsistent offsets", who);
-  }
-  if (h->prob_in_off[P] != h->n_in_total || h->prob_ep_off[P] != h->n_ep_total ||
-      h->ep_out_off[h->n_ep_total] != h->n_out_total)
-    return fail(TW_ERR_INVALID, "%s: totals inconsistent", who);
-  return TW_OK;
-}
-
 int tw_ground_truth(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const tw_trace_keys* keys,
                     const int32_t* host_trace_n, int32_t* truth_out, void* stream_) {
   if (!eng || !dev || !keys || !host_trace_n || !truth_out) return fail(TW_ERR_INVALID, "tw_ground_truth: NULL argument");
-  int rc = offsets_ok(h, "tw_ground_truth");
+  int rc = validate_host(h, "tw_ground_truth", false, false);
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream_;
   CU(cudaSetDevice(eng->device));
@@ -515,33 +487,31 @@ int tw_ground_truth(tw_engine* eng, const tw_batch* dev, const tw_batch* h, cons
     tab_off[p + 1] = tab_off[p] + (int64_t)(h->prob_ep_off[p + 1] - h->prob_ep_off[p]) * host_trace_n[p];
   }
   if (tab_off[P] > (int64_t)1 << 32) return fail(TW_ERR_RANGE_LIMIT, "tw_ground_truth: trace numbers of a service are too sparse");
-  CU(eng->alloc(&eng->truth_tab, (size_t)tab_off[P]));
-  CU(eng->alloc(&eng->truth_tab_off, (size_t)P + 1));
-  CU(eng->alloc(&eng->in_prob, (size_t)h->n_in_total));
-  CU(cudaMemcpyAsync(eng->truth_tab_off, tab_off.data(), tab_off.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
-  CU(launch_in_prob(*dev, eng->in_prob, s));
-  CU(launch_ground_truth(*dev, keys->in_trace, keys->out_trace, keys->prob_trace_lo, keys->prob_trace_n, eng->truth_tab_off,
-                         tab_off[P], eng->truth_tab, eng->in_prob, truth_out, s));
+  CU(eng->truth_tab.reserve((size_t)tab_off[P]));
+  CU(eng->truth_tab_off.reserve((size_t)P + 1));
+  CU(eng->in_prob.reserve((size_t)h->n_in_total));
+  CU(cudaMemcpyAsync(eng->truth_tab_off.p, tab_off.data(), tab_off.size() * sizeof(int64_t), cudaMemcpyHostToDevice, s));
+  CU(launch_in_prob(*dev, eng->in_prob.p, s, eng->launches));
+  CU(launch_ground_truth(*dev, keys->in_trace, keys->out_trace, keys->prob_trace_lo, keys->prob_trace_n,
+                         eng->truth_tab_off.p, tab_off[P], eng->truth_tab.p, eng->in_prob.p, truth_out, s, eng->launches));
   CU(cudaStreamSynchronize(s));    // tab_off goes out of scope
-  eng->launches += 3;
   return TW_OK;
 }
 
 int tw_find_order(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const int32_t* truth, uint32_t* violated_out,
                   void* stream_) {
   if (!eng || !dev || !truth || !violated_out) return fail(TW_ERR_INVALID, "tw_find_order: NULL argument");
-  int rc = offsets_ok(h, "tw_find_order");
+  int rc = validate_host(h, "tw_find_order", false, false);
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream_;
   CU(cudaSetDevice(eng->device));
-  CU(eng->alloc(&eng->in_prob, (size_t)h->n_in_total));
-  CU(eng->alloc(&eng->order_missing, 1));
-  CU(launch_in_prob(*dev, eng->in_prob, s));
-  CU(launch_find_order(*dev, truth, eng->in_prob, violated_out, eng->order_missing, s));
+  CU(eng->in_prob.reserve((size_t)h->n_in_total));
+  CU(eng->order_missing.reserve(1));
+  CU(launch_in_prob(*dev, eng->in_prob.p, s, eng->launches));
+  CU(launch_find_order(*dev, truth, eng->in_prob.p, violated_out, eng->order_missing.p, s, eng->launches));
   int missing = 0;
-  CU(cudaMemcpyAsync(&missing, eng->order_missing, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(&missing, eng->order_missing.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));
-  eng->launches += 2;
   if (missing) return fail(TW_ERR_INVALID, "tw_find_order: an incoming span has no child at some callee%s", "");
   return TW_OK;
 }
@@ -551,23 +521,22 @@ int tw_accuracy(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const in
                 const uint8_t* prob_first, uint64_t* per_prob_out, uint64_t* e2e_out, void* stream_) {
   if (!eng || !dev || !truth || !assign || !per_prob_out || !e2e_out) return fail(TW_ERR_INVALID, "tw_accuracy: NULL argument");
   if ((topk_idx != nullptr) != (topk_cnt != nullptr)) return fail(TW_ERR_INVALID, "tw_accuracy: topk_idx and topk_cnt go together");
-  int rc = offsets_ok(h, "tw_accuracy");
+  int rc = validate_host(h, "tw_accuracy", false, false);
   if (rc) return rc;
   if (n_traces < 0 || !in_trace) n_traces = 0;
   cudaStream_t s = (cudaStream_t)stream_;
   CU(cudaSetDevice(eng->device));
-  CU(eng->alloc(&eng->in_prob, (size_t)h->n_in_total));
-  CU(eng->alloc(&eng->acc_flags, (size_t)3 * (size_t)n_traces + 8));
-  CU(eng->alloc(&eng->acc_first, (size_t)n_traces + 1));
-  CU(cudaMemsetAsync(eng->acc_flags, 0, (size_t)3 * (size_t)n_traces + 1, s));
-  CU(cudaMemsetAsync(eng->acc_first, 0, ((size_t)n_traces + 1) * sizeof(unsigned long long), s));
+  CU(eng->in_prob.reserve((size_t)h->n_in_total));
+  CU(eng->acc_flags.reserve((size_t)3 * (size_t)n_traces + 8));
+  CU(eng->acc_first.reserve((size_t)n_traces + 1));
+  CU(cudaMemsetAsync(eng->acc_flags.p, 0, (size_t)3 * (size_t)n_traces + 1, s));
+  CU(cudaMemsetAsync(eng->acc_first.p, 0, ((size_t)n_traces + 1) * sizeof(unsigned long long), s));
   CU(cudaMemsetAsync(per_prob_out, 0, (size_t)h->n_problems * 2 * sizeof(uint64_t), s));
   CU(cudaMemsetAsync(e2e_out, 0, 4 * sizeof(uint64_t), s));
-  CU(launch_in_prob(*dev, eng->in_prob, s));
-  CU(launch_accuracy(*dev, truth, assign, topk_idx, topk_cnt, n_traces ? in_trace : nullptr, eng->in_prob, prob_first,
-                     n_traces, (unsigned long long*)per_prob_out, eng->acc_flags, eng->acc_first,
-                     (unsigned long long*)e2e_out, s));
-  eng->launches += 3;
+  CU(launch_in_prob(*dev, eng->in_prob.p, s, eng->launches));
+  CU(launch_accuracy(*dev, truth, assign, topk_idx, topk_cnt, n_traces ? in_trace : nullptr, eng->in_prob.p, prob_first,
+                     n_traces, (unsigned long long*)per_prob_out, eng->acc_flags.p, eng->acc_first.p,
+                     (unsigned long long*)e2e_out, s, eng->launches));
   return TW_OK;
 }
 
@@ -581,9 +550,8 @@ static int need_bound(tw_engine* eng, const char* who) {
 int tw_params_pass0(tw_engine* eng, const int64_t* prob_gauss_off, double* gauss_out, void* stream) {
   int rc = need_bound(eng, "tw_params_pass0");
   if (rc) return rc;
-  CU(launch_params0(eng->dev, eng->in_end_sorted, eng->out_end_sorted, prob_gauss_off, eng->batch_prob,
-                    eng->batch_idx, eng->n_batches_total, gauss_out, (cudaStream_t)stream));
-  eng->launches += 1;
+  CU(launch_params0(eng->dev, eng->in_end_sorted.p, eng->out_end_sorted.p, prob_gauss_off, eng->batch_prob.p,
+                    eng->batch_idx.p, eng->n_batches_total, gauss_out, (cudaStream_t)stream, eng->launches));
   return TW_OK;
 }
 
@@ -603,34 +571,31 @@ int tw_score_topk(tw_engine* eng, const tw_params* params, const tw_score_out* o
   tw_score_out o = *out;
   if (!o.used_lo) {                    // the perfect-cut pass reads the maps: keep them in engine scratch
     const size_t nt = (size_t)eng->dev_n_tuple;
-    CU(eng->alloc(&eng->own_used_lo, nt));
-    CU(eng->alloc(&eng->own_used_bits, 2 * nt));
-    CU(eng->alloc(&eng->own_used_wide, (size_t)eng->dev.n_in_total));
-    o.used_lo = eng->own_used_lo;
-    o.used_bits = eng->own_used_bits;
-    o.used_wide = eng->own_used_wide;
+    CU(eng->own_used_lo.reserve(nt));
+    CU(eng->own_used_bits.reserve(2 * nt));
+    CU(eng->own_used_wide.reserve((size_t)eng->dev.n_in_total));
+    o.used_lo = eng->own_used_lo.p;
+    o.used_bits = eng->own_used_bits.p;
+    o.used_wide = eng->own_used_wide.p;
   }
   ScoreTiles st;
-  st.tile_prob = eng->score_tiles;
-  st.tile_start = eng->score_tiles + eng->n_tiles;
-  st.tile_win = eng->tile_win;
-  st.overflow = eng->tile_overflow;
+  st.tile_prob = eng->score_tiles.p;
+  st.tile_start = eng->score_tiles.p + eng->n_tiles;
+  st.tile_win = eng->tile_win.p;
+  st.overflow = eng->tile_overflow.p;
   st.n_tiles = eng->n_tiles;
   for (int q = 0; q <= TW_MAX_E; ++q) st.class_off[q] = eng->class_off[q];
-  TileList wide{eng->wide_tiles, eng->wide_tiles + eng->n_wide, eng->n_wide, kWideThreads - 1,
-                eng->wide_tiles + 3 * eng->n_wide};
-  int nl = 0;
+  TileList wide{eng->wide_tiles.p, eng->wide_tiles.p + eng->n_wide, eng->n_wide, kWideThreads - 1,
+                eng->wide_tiles.p + 3 * eng->n_wide};
   // work-balanced scoring kernel (one launch per E present); flagged tiles are redone by the
   // sequential kernel; PerfectCut flags from the candidate maps
-  CU(launch_score3(eng->dev, params, o, keep, st, eng->prev_idx, eng->device, &nl, s));
-  CU(launch_score_redo(eng->dev, params, o, wide, eng->prev_idx, eng->tile_overflow, eng->device, eng->err_flag, s));
-  ++nl;
+  CU(launch_score3(eng->dev, params, o, keep, st, eng->prev_idx.p, s, eng->launches));
+  CU(launch_score_redo(eng->dev, params, o, wide, eng->prev_idx.p, eng->tile_overflow.p, eng->n_sm, eng->err_flag.p, s,
+                       eng->launches));
   if (!keep) {
-    CU(launch_cut(eng->dev, o, st, eng->prev_idx, s));
-    ++nl;
+    CU(launch_cut(eng->dev, o, st, eng->prev_idx.p, s, eng->launches));
     eng->windows_valid = true;
   }
-  eng->launches += nl;
   return TW_OK;
 }
 
@@ -649,10 +614,9 @@ int tw_stitch(tw_engine* eng, const tw_params* params, const uint8_t* cut, const
       return fail(TW_ERR_INVALID, "tw_stitch: `undeleted` needs top-K, n_feasible and the used maps");
     spec = *undeleted;
   }
-  StitchUnits ub{eng->unit_prob, eng->unit_lo, eng->unit_hi, eng->unit_count};
-  CU(launch_stitch(eng->dev, *params, cut, spec, *out, eng->taken, eng->taken_words, eng->node_limit, ub, eng->max_units,
-                   eng->device, eng->err_flag, (cudaStream_t)stream));
-  eng->launches += (undeleted && eng->dev.n_problems < kStitchUnitMaxServices) ? 2 : 1;
+  StitchUnits ub{eng->unit_prob.p, eng->unit_lo.p, eng->unit_hi.p, eng->unit_count.p};
+  CU(launch_stitch(eng->dev, *params, cut, spec, *out, eng->taken.p, eng->taken_words, eng->node_limit, ub,
+                   eng->max_units, eng->err_flag.p, (cudaStream_t)stream, eng->launches));
   return TW_OK;
 }
 
@@ -660,9 +624,8 @@ int tw_delays(tw_engine* eng, const int32_t* assign, const int64_t* term_sample_
               int32_t* counts, void* stream) {
   int rc = need_bound(eng, "tw_delays");
   if (rc) return rc;
-  CU(launch_delays(eng->dev, assign, term_sample_off, eng->term_ep, eng->ep_prob, delays, counts,
-                   (cudaStream_t)stream));
-  eng->launches += 1;
+  CU(launch_delays(eng->dev, assign, term_sample_off, eng->term_ep.p, eng->ep_prob.p, delays, counts,
+                   (cudaStream_t)stream, eng->launches));
   return TW_OK;
 }
 
@@ -679,11 +642,11 @@ static void numpy_random_samples(uint32_t seed, int count, std::vector<double>& 
 
 static int gmm_prepare(tw_engine* eng, uint32_t seed_select, cudaStream_t s) {
   const int nt = eng->dev.n_term_total;
-  CU(eng->alloc(&eng->gmm_max_n, (size_t)nt));
-  CU(eng->alloc(&eng->gmm_mean_var, (size_t)nt * 2));
-  CU(eng->alloc(&eng->gmm_skip, (size_t)nt + 64));   // + histogram / cursors of the final-fit grouping
-  CU(eng->alloc(&eng->gmm_bic, (size_t)nt * TW_GMM_MAX_COMP));
-  CU(eng->alloc(&eng->gmm_cen, (size_t)nt * TW_GMM_MAX_COMP * TW_GMM_MAX_COMP));   // one slab per K
+  CU(eng->gmm_max_n.reserve((size_t)nt));
+  CU(eng->gmm_mean_var.reserve((size_t)nt * 2));
+  CU(eng->gmm_skip.reserve((size_t)nt + 64));   // + histogram / cursors of the final-fit grouping
+  CU(eng->gmm_bic.reserve((size_t)nt * TW_GMM_MAX_COMP));
+  CU(eng->gmm_cen.reserve((size_t)nt * TW_GMM_MAX_COMP * TW_GMM_MAX_COMP));   // one slab per K
   if (!eng->gmm_fork.ready) {
     CU(cudaEventCreateWithFlags(&eng->gmm_fork.fork, cudaEventDisableTiming));
     for (int q = 0; q < TW_GMM_MAX_COMP; ++q) {
@@ -692,19 +655,19 @@ static int gmm_prepare(tw_engine* eng, uint32_t seed_select, cudaStream_t s) {
     }
     eng->gmm_fork.ready = true;
   }
-  CU(eng->alloc(&eng->gmm_stream, (size_t)tw_engine::kStreamLen));
-  CU(eng->alloc(&eng->gmm_stream100, 16));
+  CU(eng->gmm_stream.reserve((size_t)tw_engine::kStreamLen, &eng->gmm_seed_valid));
+  CU(eng->gmm_stream100.reserve(16, &eng->gmm_stream100_valid));
   if (!eng->gmm_stream100_valid) {
     std::vector<double> s100;
     numpy_random_samples(100u, 16, s100);
-    CU(cudaMemcpyAsync(eng->gmm_stream100, s100.data(), 16 * sizeof(double), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(eng->gmm_stream100.p, s100.data(), 16 * sizeof(double), cudaMemcpyHostToDevice, s));
     CU(cudaStreamSynchronize(s));
     eng->gmm_stream100_valid = true;
   }
   if (!eng->gmm_seed_valid || eng->gmm_seed != seed_select) {
     std::vector<double> st;
     numpy_random_samples(seed_select, tw_engine::kStreamLen, st);
-    CU(cudaMemcpyAsync(eng->gmm_stream, st.data(), st.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(eng->gmm_stream.p, st.data(), st.size() * sizeof(double), cudaMemcpyHostToDevice, s));
     CU(cudaStreamSynchronize(s));
     eng->gmm_seed = seed_select;
     eng->gmm_seed_valid = true;
@@ -722,13 +685,12 @@ int tw_gmm_refit(tw_engine* eng, const int64_t* term_sample_off, const double* d
   rc = gmm_prepare(eng, seed_select, s);
   if (rc) return rc;
   const int nt = eng->dev.n_term_total;
-  CU(launch_gmm_prep(nt, term_sample_off, delays, counts, eng->gmm_max_n, eng->gmm_mean_var, s));
-  CU(launch_gmm_skip(eng->dev.n_problems, eng->dev.prob_ep_off, eng->dev.ep_term_off, term_order, eng->gmm_max_n,
-                     prob_base_skip, eng->gmm_skip, s));
-  CU(launch_gmm_fit(nt, term_sample_off, delays, counts, eng->gmm_max_n, eng->gmm_mean_var, eng->gmm_skip,
-                    eng->gmm_stream, tw_engine::kStreamLen, eng->gmm_stream100, eng->gmm_bic, eng->gmm_cen,
-                    mix_out, n_selected_out, eng->err_flag, &eng->gmm_fork, s));
-  eng->launches += 34;   // prep, skip, 5 x (seed, lloyd, bic), select, group, 5 x (seed, lloyd, final)
+  CU(launch_gmm_prep(nt, term_sample_off, delays, counts, eng->gmm_max_n.p, eng->gmm_mean_var.p, s, eng->launches));
+  CU(launch_gmm_skip(eng->dev.n_problems, eng->dev.prob_ep_off, eng->dev.ep_term_off, term_order, eng->gmm_max_n.p,
+                     prob_base_skip, eng->gmm_skip.p, s, eng->launches));
+  CU(launch_gmm_fit(nt, term_sample_off, delays, counts, eng->gmm_max_n.p, eng->gmm_mean_var.p, eng->gmm_skip.p,
+                    eng->gmm_stream.p, tw_engine::kStreamLen, eng->gmm_stream100.p, eng->gmm_bic.p, eng->gmm_cen.p,
+                    mix_out, n_selected_out, eng->err_flag.p, &eng->gmm_fork, s, eng->launches));
   return TW_OK;
 }
 
@@ -742,10 +704,9 @@ int tw_gmm_stream_draws(tw_engine* eng, const int64_t* term_sample_off, const do
   rc = gmm_prepare(eng, eng->gmm_seed_valid ? eng->gmm_seed : 10u, s);
   if (rc) return rc;
   const int nt = eng->dev.n_term_total;
-  CU(launch_gmm_prep(nt, term_sample_off, delays, counts, eng->gmm_max_n, eng->gmm_mean_var, s));
-  CU(launch_gmm_draws(eng->dev.n_problems, eng->dev.prob_ep_off, eng->dev.ep_term_off, eng->gmm_max_n,
-                      prob_draws_out, s));
-  eng->launches += 2;
+  CU(launch_gmm_prep(nt, term_sample_off, delays, counts, eng->gmm_max_n.p, eng->gmm_mean_var.p, s, eng->launches));
+  CU(launch_gmm_draws(eng->dev.n_problems, eng->dev.prob_ep_off, eng->dev.ep_term_off, eng->gmm_max_n.p,
+                      prob_draws_out, s, eng->launches));
   return TW_OK;
 }
 

@@ -834,9 +834,9 @@ k_fp64_peak(int iters, double* __restrict__ sink) {
   if (r == 123.456) sink[0] = r;       // never true: keeps the chains alive
 }
 
-cudaError_t launch_fp64_peak(int blocks, int iters, double* sink, cudaStream_t s) {
+cudaError_t launch_fp64_peak(int blocks, int iters, double* sink, cudaStream_t s, int64_t& launches) {
   k_fp64_peak<<<blocks, 256, 0, s>>>(iters, sink);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 cudaError_t gmm_work_read(unsigned long long* out, bool reset) {
@@ -862,35 +862,36 @@ extern "C" int tw_debug_gmm_phases(unsigned long long* out16, int reset) {
 #endif
 
 cudaError_t launch_gmm_prep(int n_terms, const int64_t* term_sample_off, const double* delays,
-                            const int32_t* counts, int32_t* max_n, double* mean_var, cudaStream_t s) {
+                            const int32_t* counts, int32_t* max_n, double* mean_var, cudaStream_t s,
+                            int64_t& launches) {
   k_gmm_prep<<<(n_terms + 3) / 4, 128, 0, s>>>(n_terms, term_sample_off, delays, counts, max_n, mean_var);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 cudaError_t launch_gmm_skip(int n_problems, const int32_t* prob_ep_off, const int32_t* ep_term_off,
                             const int32_t* term_order, const int32_t* max_n, const uint32_t* prob_base_skip,
-                            uint32_t* rng_skip, cudaStream_t s) {
+                            uint32_t* rng_skip, cudaStream_t s, int64_t& launches) {
   k_gmm_skip<<<(n_problems + 127) / 128, 128, 0, s>>>(n_problems, prob_ep_off, ep_term_off, term_order, max_n,
                                                        prob_base_skip, rng_skip);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 cudaError_t launch_gmm_draws(int n_problems, const int32_t* prob_ep_off, const int32_t* ep_term_off,
-                             const int32_t* max_n, uint32_t* prob_draws, cudaStream_t s) {
+                             const int32_t* max_n, uint32_t* prob_draws, cudaStream_t s, int64_t& launches) {
   k_gmm_draws<<<(n_problems + 127) / 128, 128, 0, s>>>(n_problems, prob_ep_off, ep_term_off, max_n, prob_draws);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 template <int K>
 static cudaError_t launch_fit_phases(const FitSel& sel, int n_warps, const int64_t* term_sample_off,
                                      const double* delays, const int32_t* counts, const double* mean_var,
-                                     double* cen, int* err_flag, cudaStream_t s) {
+                                     double* cen, int* err_flag, cudaStream_t s, int64_t& launches) {
   const int blocks = (n_warps + 3) / 4;
   k_gmm_seed<K><<<blocks, 128, 0, s>>>(sel, term_sample_off, delays, counts, mean_var, cen, err_flag);
-  cudaError_t e = cudaGetLastError();
+  cudaError_t e = after_launch(launches);
   if (e != cudaSuccess) return e;
   k_gmm_lloyd<K><<<blocks, 128, 0, s>>>(sel, term_sample_off, delays, counts, mean_var, cen);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 // fork: every side stream waits for the work queued on s so far; join: s waits for every side stream
@@ -916,7 +917,8 @@ cudaError_t launch_gmm_fit(int n_terms, const int64_t* term_sample_off, const do
                            const int32_t* counts, const int32_t* max_n, const double* mean_var,
                            const uint32_t* rng_skip, const double* stream, int stream_len,
                            const double* stream100, double* bic, double* cen, double* mix_out,
-                           int32_t* n_selected_out, int* err_flag, GmmFork* fk, cudaStream_t s) {
+                           int32_t* n_selected_out, int* err_flag, GmmFork* fk, cudaStream_t s,
+                           int64_t& launches) {
   cudaError_t e;
   const int blocks = (n_terms + 3) / 4;
   const size_t slab = (size_t)n_terms * KC;
@@ -927,10 +929,11 @@ cudaError_t launch_gmm_fit(int n_terms, const int64_t* term_sample_off, const do
   {                                                                                                        \
     cudaStream_t q = fk->side[K - 1];                                                                      \
     double* c = cen + (K - 1) * slab;                                                                      \
-    e = launch_fit_phases<K>(sel, n_terms, term_sample_off, delays, counts, mean_var, c, err_flag, q);     \
+    e = launch_fit_phases<K>(sel, n_terms, term_sample_off, delays, counts, mean_var, c, err_flag, q,      \
+                             launches);                                                                    \
     if (e != cudaSuccess) return e;                                                                        \
     k_gmm_bic<K><<<blocks, 128, 0, q>>>(sel, term_sample_off, delays, counts, mean_var, c, bic);           \
-    e = cudaGetLastError();                                                                                \
+    e = after_launch(launches);                                                                            \
     if (e != cudaSuccess) return e;                                                                        \
   }
   TW_BIC(5) TW_BIC(4) TW_BIC(3) TW_BIC(2) TW_BIC(1)     // longest fits first
@@ -947,10 +950,10 @@ cudaError_t launch_gmm_fit(int n_terms, const int64_t* term_sample_off, const do
   e = cudaMemsetAsync(hist, 0, 16 * sizeof(uint32_t), s);
   if (e != cudaSuccess) return e;
   k_gmm_select<<<(n_terms + 127) / 128, 128, 0, s>>>(n_terms, max_n, bic, best_k, hist, mix_out, n_selected_out);
-  e = cudaGetLastError();
+  e = after_launch(launches);
   if (e != cudaSuccess) return e;
   k_gmm_group<<<(n_terms + 127) / 128, 128, 0, s>>>(n_terms, best_k, hist, cursor, list);
-  e = cudaGetLastError();
+  e = after_launch(launches);
   if (e != cudaSuccess) return e;
   const FitSel fin{list, hist, nullptr, nullptr, stream100, 16, n_terms};
   e = fork_streams(fk, s);
@@ -959,11 +962,12 @@ cudaError_t launch_gmm_fit(int n_terms, const int64_t* term_sample_off, const do
   {                                                                                                        \
     cudaStream_t q = fk->side[K - 1];                                                                      \
     double* c = cen + (K - 1) * slab;                                                                      \
-    e = launch_fit_phases<K>(fin, n_terms, term_sample_off, delays, counts, mean_var, c, nullptr, q);      \
+    e = launch_fit_phases<K>(fin, n_terms, term_sample_off, delays, counts, mean_var, c, nullptr, q,       \
+                             launches);                                                                    \
     if (e != cudaSuccess) return e;                                                                        \
     k_gmm_final<K><<<blocks, 128, 0, q>>>(fin, term_sample_off, delays, counts, mean_var, c, mix_out,      \
                                           n_selected_out);                                                 \
-    e = cudaGetLastError();                                                                                \
+    e = after_launch(launches);                                                                            \
     if (e != cudaSuccess) return e;                                                                        \
   }
   TW_FINAL(5) TW_FINAL(4) TW_FINAL(3) TW_FINAL(2) TW_FINAL(1)

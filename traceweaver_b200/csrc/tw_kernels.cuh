@@ -26,8 +26,6 @@ constexpr int kWideThreads = 32;                 // (31 in-spans + carry-in per 
 // ---- stitch kernel geometry (tw_stitch.cu) --------------------------------------------------
 constexpr int kStitchWarps = 2;                  // one warp per problem
 
-struct EngineScratch;                            // tw_api.cu
-
 // Tiles: a tile never crosses a problem.  tile_prob[t], tile_start[t] (problem-local in-span).
 struct TileList {
   const int32_t* tile_prob;
@@ -48,17 +46,31 @@ struct ScoreTiles {
   int class_off[TW_MAX_E + 1];
 };
 
-cudaError_t launch_prev_index(const tw_batch& b, int32_t* prev_idx, cudaStream_t s);
-cudaError_t launch_tile_meta(const tw_batch& b, const TileList& tiles, int32_t* tile_win, cudaStream_t s);
+// Kernels launched with more than 48 KB of dynamic shared memory need the limit raised once per
+// device: tw_engine_create calls these for the engine's device.
+cudaError_t setup_score3();                      // k_score3<1..TW_MAX_E>
+cudaError_t setup_score();                       // k_score<kWideThreads, kWideW>
+cudaError_t setup_stitch();                      // k_stitch
+cudaError_t setup_sort_ends();                   // k_sort_ends
+
+// Every launch_* function adds the kernels it issues to `launches` (tw_engine_launch_count):
+// after_launch directly follows each <<<...>>>, counts it if it was issued and returns its error.
+inline cudaError_t after_launch(int64_t& launches) {
+  const cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) ++launches;
+  return e;
+}
+cudaError_t launch_prev_index(const tw_batch& b, int32_t* prev_idx, cudaStream_t s, int64_t& launches);
+cudaError_t launch_tile_meta(const tw_batch& b, const TileList& tiles, int32_t* tile_win, cudaStream_t s,
+                             int64_t& launches);
 cudaError_t launch_score3(const tw_batch& b, const tw_params* prm, const tw_score_out& out, int keep_windows,
-                          const ScoreTiles& st, const int32_t* prev_idx, int device, int* n_launches,
-                          cudaStream_t s);
+                          const ScoreTiles& st, const int32_t* prev_idx, cudaStream_t s, int64_t& launches);
 cudaError_t launch_cut(const tw_batch& b, const tw_score_out& out, const ScoreTiles& st, const int32_t* prev_idx,
-                       cudaStream_t s);
+                       cudaStream_t s, int64_t& launches);
 // sequential redo of the tiles the scoring kernel flagged (wide tiles subdivide scoring tiles)
 cudaError_t launch_score_redo(const tw_batch& b, const tw_params* prm, const tw_score_out& out,
                               const TileList& wide, const int32_t* prev_idx, uint8_t* tile_overflow,
-                              int device, int* err_flag, cudaStream_t s);
+                              int n_sm, int* err_flag, cudaStream_t s, int64_t& launches);
 // units of the stitch kernel (tw_stitch.cu: k_stitch_units): unit u = in-spans [lo[u], hi[u]) of service prob[u]
 struct StitchUnits {
   int32_t* prob;
@@ -70,56 +82,70 @@ constexpr int kStitchUnitMin = 48;               // a unit is closed at the firs
 constexpr int kStitchUnitMaxServices = 4096;     // batches with at least this many services keep one warp per service
 cudaError_t launch_stitch(const tw_batch& b, const tw_params& prm, const uint8_t* cut,
                           const tw_score_out& spec, const tw_pass_out& out, uint32_t* taken_words, size_t taken_n_words,
-                          long long node_limit, const StitchUnits& unit_buf, int max_units, int device, int* err_flag,
-                          cudaStream_t s);
+                          long long node_limit, const StitchUnits& unit_buf, int max_units, int* err_flag,
+                          cudaStream_t s, int64_t& launches);
 constexpr int kSortSmemCap = 16384;               // longest list the shared-memory sort network takes
 cudaError_t launch_sort_ends(const tw_batch& b, int64_t* in_end_sorted, int64_t* out_end_sorted,
                              int max_seg, const int32_t* long_seg, int n_long, int64_t* long_scratch,
-                             int64_t slab_len, int* err_flag, cudaStream_t s);
+                             int64_t slab_len, int* err_flag, cudaStream_t s, int64_t& launches);
 cudaError_t launch_params0(const tw_batch& b, const int64_t* in_end_sorted,
                            const int64_t* out_end_sorted, const int64_t* prob_gauss_off,
                            const int32_t* batch_prob, const int32_t* batch_idx, int n_batches_total,
-                           double* gauss_out, cudaStream_t s);
+                           double* gauss_out, cudaStream_t s, int64_t& launches);
 cudaError_t launch_delays(const tw_batch& b, const int32_t* assign, const int64_t* term_sample_off,
                           const int32_t* term_ep, const int32_t* ep_prob, double* delays,
-                          int32_t* counts, cudaStream_t s);
+                          int32_t* counts, cudaStream_t s, int64_t& launches);
 
 cudaError_t launch_gmm_prep(int n_terms, const int64_t* term_sample_off, const double* delays,
-                            const int32_t* counts, int32_t* max_n, double* mean_var, cudaStream_t s);
+                            const int32_t* counts, int32_t* max_n, double* mean_var, cudaStream_t s,
+                            int64_t& launches);
 cudaError_t launch_gmm_skip(int n_problems, const int32_t* prob_ep_off, const int32_t* ep_term_off,
                             const int32_t* term_order, const int32_t* max_n,
-                            const uint32_t* prob_base_skip, uint32_t* rng_skip, cudaStream_t s);
+                            const uint32_t* prob_base_skip, uint32_t* rng_skip, cudaStream_t s, int64_t& launches);
 cudaError_t launch_gmm_draws(int n_problems, const int32_t* prob_ep_off, const int32_t* ep_term_off,
-                             const int32_t* max_n, uint32_t* prob_draws, cudaStream_t s);
+                             const int32_t* max_n, uint32_t* prob_draws, cudaStream_t s, int64_t& launches);
 // side streams + events of the refit: the five per-K fit chains are independent and run concurrently
 struct GmmFork {
-  cudaStream_t side[TW_GMM_MAX_COMP];
-  cudaEvent_t fork, join[TW_GMM_MAX_COMP];
+  cudaStream_t side[TW_GMM_MAX_COMP] = {};
+  cudaEvent_t fork = nullptr, join[TW_GMM_MAX_COMP] = {};
   bool ready = false;
+  GmmFork() = default;
+  GmmFork(const GmmFork&) = delete;
+  GmmFork& operator=(const GmmFork&) = delete;
+  ~GmmFork() {
+    if (fork) cudaEventDestroy(fork);
+    for (int q = 0; q < TW_GMM_MAX_COMP; ++q) {
+      if (join[q]) cudaEventDestroy(join[q]);
+      if (side[q]) cudaStreamDestroy(side[q]);
+    }
+  }
 };
 cudaError_t launch_gmm_fit(int n_terms, const int64_t* term_sample_off, const double* delays,
                            const int32_t* counts, const int32_t* max_n, const double* mean_var,
                            const uint32_t* rng_skip, const double* stream, int stream_len,
                            const double* stream100, double* bic, double* cen, double* mix_out,
-                           int32_t* n_selected_out, int* err_flag, GmmFork* fk, cudaStream_t s);
+                           int32_t* n_selected_out, int* err_flag, GmmFork* fk, cudaStream_t s,
+                           int64_t& launches);
 
 cudaError_t launch_skip(const tw_batch& b, const tw_skip_desc& sd, const tw_skip_out& out, uint32_t* taken,
                         uint32_t* set_scratch, const int64_t* prob_set_off, int32_t* win_scratch,
-                        long long node_limit, int* err_flag, cudaStream_t s);
+                        long long node_limit, int* err_flag, cudaStream_t s, int64_t& launches);
 cudaError_t launch_build_dist(int n, const int64_t* ms, const int64_t* me, const int8_t* label, int E,
-                              int64_t large_delay, int32_t* key, int64_t* val, cudaStream_t s);
+                              int64_t large_delay, int32_t* key, int64_t* val, cudaStream_t s, int64_t& launches);
 
-cudaError_t launch_fp64_peak(int blocks, int iters, double* sink, cudaStream_t s);
+cudaError_t launch_fp64_peak(int blocks, int iters, double* sink, cudaStream_t s, int64_t& launches);
 cudaError_t gmm_work_read(unsigned long long* out, bool reset);
-cudaError_t launch_in_prob(const tw_batch& b, int32_t* in_prob, cudaStream_t s);
+cudaError_t launch_in_prob(const tw_batch& b, int32_t* in_prob, cudaStream_t s, int64_t& launches);
 cudaError_t launch_ground_truth(const tw_batch& b, const int32_t* in_trace, const int32_t* out_trace,
                                 const int32_t* trace_lo, const int32_t* trace_n, const int64_t* tab_off, int64_t tab_len,
-                                int32_t* tab, const int32_t* in_prob, int32_t* truth, cudaStream_t s);
+                                int32_t* tab, const int32_t* in_prob, int32_t* truth, cudaStream_t s,
+                                int64_t& launches);
 cudaError_t launch_find_order(const tw_batch& b, const int32_t* truth, const int32_t* in_prob, uint32_t* violated,
-                              int* missing, cudaStream_t s);
+                              int* missing, cudaStream_t s, int64_t& launches);
 cudaError_t launch_accuracy(const tw_batch& b, const int32_t* truth, const int32_t* assign, const int32_t* topk_idx,
                             const uint8_t* topk_cnt, const int32_t* in_trace, const int32_t* in_prob,
                             const uint8_t* prob_first, int n_traces, unsigned long long* per_prob, uint8_t* flags,
-                            unsigned long long* trace_first, unsigned long long* out4, cudaStream_t s);
+                            unsigned long long* trace_first, unsigned long long* out4, cudaStream_t s,
+                            int64_t& launches);
 
 }  // namespace tw

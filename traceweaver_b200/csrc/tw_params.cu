@@ -100,21 +100,24 @@ k_sort_ends_long(tw_batch b, const int32_t* __restrict__ long_seg, int64_t* __re
   for (int x = threadIdx.x; x < n; x += blockDim.x) dst[x] = a[x];
 }
 
+cudaError_t setup_sort_ends() {
+  return cudaFuncSetAttribute(k_sort_ends, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)(kSortSmemCap * sizeof(int64_t)));
+}
+
 cudaError_t launch_sort_ends(const tw_batch& b, int64_t* in_end_sorted, int64_t* out_end_sorted,
                              int max_seg, const int32_t* long_seg, int n_long, int64_t* long_scratch,
-                             int64_t slab_len, int* err_flag, cudaStream_t s) {
+                             int64_t slab_len, int* err_flag, cudaStream_t s, int64_t& launches) {
   int cap = 1;
   while (cap < max_seg && cap < kSortSmemCap) cap <<= 1;
   size_t smem = (size_t)cap * sizeof(int64_t);
-  cudaError_t e = cudaFuncSetAttribute(k_sort_ends, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return e;
   k_sort_ends<<<b.n_problems + b.n_ep_total, kSortThreads, smem, s>>>(b, in_end_sorted, out_end_sorted, cap,
                                                                        err_flag);
-  e = cudaGetLastError();
+  cudaError_t e = after_launch(launches);
   if (e != cudaSuccess) return e;
   if (n_long > 0) {
     k_sort_ends_long<<<n_long, 1024, 0, s>>>(b, long_seg, long_scratch, slab_len, in_end_sorted, out_end_sorted);
-    e = cudaGetLastError();
+    e = after_launch(launches);
   }
   return e;
 }
@@ -211,11 +214,11 @@ k_params0(tw_batch b, const int64_t* __restrict__ in_end_sorted, const int64_t* 
 
 cudaError_t launch_params0(const tw_batch& b, const int64_t* in_end_sorted, const int64_t* out_end_sorted,
                            const int64_t* prob_gauss_off, const int32_t* batch_prob, const int32_t* batch_idx,
-                           int n_batches_total, double* gauss_out, cudaStream_t s) {
+                           int n_batches_total, double* gauss_out, cudaStream_t s, int64_t& launches) {
   int blocks = (n_batches_total + 3) / 4;
   k_params0<<<blocks, 128, 0, s>>>(b, in_end_sorted, out_end_sorted, prob_gauss_off, batch_prob, batch_idx,
                                    n_batches_total, gauss_out);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -267,10 +270,10 @@ k_delays(tw_batch b, const int32_t* __restrict__ assign, const int64_t* __restri
 
 cudaError_t launch_delays(const tw_batch& b, const int32_t* assign, const int64_t* term_sample_off,
                           const int32_t* term_ep, const int32_t* ep_prob, double* delays, int32_t* counts,
-                          cudaStream_t s) {
+                          cudaStream_t s, int64_t& launches) {
   int blocks = (b.n_term_total + 3) / 4;
   k_delays<<<blocks, 128, 0, s>>>(b, assign, term_sample_off, term_ep, ep_prob, delays, counts);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 }  // namespace tw

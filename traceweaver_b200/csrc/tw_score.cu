@@ -57,11 +57,11 @@ __global__ void __launch_bounds__(128) k_prev_index(tw_batch b, int32_t* __restr
   }
 }
 
-cudaError_t launch_prev_index(const tw_batch& b, int32_t* prev_idx, cudaStream_t s) {
+cudaError_t launch_prev_index(const tw_batch& b, int32_t* prev_idx, cudaStream_t s, int64_t& launches) {
   int warps_per_block = 4;
   int blocks = (b.n_problems + warps_per_block - 1) / warps_per_block;
   k_prev_index<<<blocks, warps_per_block * 32, 0, s>>>(b, prev_idx);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -478,31 +478,27 @@ k_score(tw_batch b, tw_params prm, int has_params, tw_score_out out, TileList ti
   }
 }
 
+using SmW = ScoreSmem<kWideThreads, kWideW>;
+
+cudaError_t setup_score() {
+  return cudaFuncSetAttribute(k_score<kWideThreads, kWideW>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)sizeof(SmW));
+}
+
 cudaError_t launch_score_redo(const tw_batch& b, const tw_params* prm, const tw_score_out& out,
                               const TileList& wide, const int32_t* prev_idx, uint8_t* tile_overflow,
-                              int device, int* err_flag, cudaStream_t s) {
+                              int n_sm, int* err_flag, cudaStream_t s, int64_t& launches) {
   tw_params dummy;
   dummy.mode = TW_PARAMS_MIXTURE; dummy.reserved0 = 0;
   dummy.prob_gauss_off = nullptr; dummy.gauss = nullptr; dummy.mix = nullptr;
   const tw_params& pr = prm ? *prm : dummy;
-  using SmW = ScoreSmem<kWideThreads, kWideW>;
-  auto kw = k_score<kWideThreads, kWideW>;
-  static bool attr_done[64] = {false};   // per device: a process may drive several GPUs
-  static int n_sm[64] = {0};
-  if (device >= 0 && device < 64 && !attr_done[device]) {
-    cudaError_t e2 = cudaFuncSetAttribute(kw, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(SmW));
-    if (e2 != cudaSuccess) return e2;
-    e2 = cudaDeviceGetAttribute(&n_sm[device], cudaDevAttrMultiProcessorCount, device);
-    if (e2 != cudaSuccess) return e2;
-    attr_done[device] = true;
-  }
   if (wide.n_tiles == 0) return cudaSuccess;
   const int chunks = (wide.n_tiles + 31) / 32;
-  const int max_grid = 16 * (device >= 0 && device < 64 ? n_sm[device] : 132);   // 16 CTAs per SM
+  const int max_grid = 16 * n_sm;   // 16 CTAs per SM
   const int wide_grid = chunks < max_grid ? chunks : max_grid;
-  kw<<<wide_grid, kWideThreads, sizeof(SmW), s>>>(b, pr, prm != nullptr, out, wide, prev_idx,
-                                                  tile_overflow, 1, err_flag);
-  return cudaGetLastError();
+  k_score<kWideThreads, kWideW><<<wide_grid, kWideThreads, sizeof(SmW), s>>>(b, pr, prm != nullptr, out, wide,
+                                                                            prev_idx, tile_overflow, 1, err_flag);
+  return after_launch(launches);
 }
 
 }  // namespace tw

@@ -815,11 +815,12 @@ k_tile_meta(tw_batch b, TileList tiles, int32_t* __restrict__ tile_win) {
   }
 }
 
-cudaError_t launch_tile_meta(const tw_batch& b, const TileList& tiles, int32_t* tile_win, cudaStream_t s) {
+cudaError_t launch_tile_meta(const tw_batch& b, const TileList& tiles, int32_t* tile_win, cudaStream_t s,
+                             int64_t& launches) {
   if (tiles.n_tiles == 0) return cudaSuccess;
   const int blocks = (tiles.n_tiles + 3) / 4;
   k_tile_meta<<<blocks, 128, 0, s>>>(b, tiles, tile_win);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -877,22 +878,26 @@ k_cut(tw_batch b, tw_score_out out, TileList tiles, const int32_t* __restrict__ 
 }
 
 template <int E>
-static cudaError_t launch_one(const tw_batch& b, const tw_params& prm, int has_params, int keep, const tw_score_out& out,
-                              const TileList& tl, const int32_t* tile_win, uint8_t* ovf, int device, cudaStream_t s) {
-  auto k = k_score3<E>;
-  static bool attr_done[64] = {false};
-  if (device >= 0 && device < 64 && !attr_done[device]) {
-    cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(S3Smem<E>));
-    if (e != cudaSuccess) return e;
-    attr_done[device] = true;
+static cudaError_t setup_from() {   // k_score3<E> .. k_score3<TW_MAX_E>
+  cudaError_t e = cudaFuncSetAttribute(k_score3<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(S3Smem<E>));
+  if constexpr (E < TW_MAX_E) {
+    if (e == cudaSuccess) e = setup_from<E + 1>();
   }
-  k<<<tl.n_tiles, kS3Threads, sizeof(S3Smem<E>), s>>>(b, prm, has_params, keep, out, tl, tile_win, ovf);
-  return cudaGetLastError();
+  return e;
+}
+
+cudaError_t setup_score3() { return setup_from<1>(); }
+
+template <int E>
+static cudaError_t launch_one(const tw_batch& b, const tw_params& prm, int has_params, int keep, const tw_score_out& out,
+                              const TileList& tl, const int32_t* tile_win, uint8_t* ovf, cudaStream_t s,
+                              int64_t& launches) {
+  k_score3<E><<<tl.n_tiles, kS3Threads, sizeof(S3Smem<E>), s>>>(b, prm, has_params, keep, out, tl, tile_win, ovf);
+  return after_launch(launches);
 }
 
 cudaError_t launch_score3(const tw_batch& b, const tw_params* prm, const tw_score_out& out, int keep_windows,
-                          const ScoreTiles& st, const int32_t* prev_idx, int device, int* n_launches,
-                          cudaStream_t s) {
+                          const ScoreTiles& st, const int32_t* prev_idx, cudaStream_t s, int64_t& launches) {
   tw_params dummy;
   dummy.mode = TW_PARAMS_MIXTURE; dummy.reserved0 = 0;
   dummy.prob_gauss_off = nullptr; dummy.gauss = nullptr; dummy.mix = nullptr;
@@ -910,26 +915,25 @@ cudaError_t launch_score3(const tw_batch& b, const tw_params* prm, const tw_scor
     const int32_t* twin = st.tile_win + (size_t)c0 * 2 * TW_MAX_E;
     uint8_t* ovf = st.overflow + c0;
     switch (E) {
-      case 1: e = launch_one<1>(b, pr, hp, keep_windows, out, tl, twin, ovf, device, s); break;
-      case 2: e = launch_one<2>(b, pr, hp, keep_windows, out, tl, twin, ovf, device, s); break;
-      case 3: e = launch_one<3>(b, pr, hp, keep_windows, out, tl, twin, ovf, device, s); break;
-      case 4: e = launch_one<4>(b, pr, hp, keep_windows, out, tl, twin, ovf, device, s); break;
-      case 5: e = launch_one<5>(b, pr, hp, keep_windows, out, tl, twin, ovf, device, s); break;
-      case 6: e = launch_one<6>(b, pr, hp, keep_windows, out, tl, twin, ovf, device, s); break;
-      case 7: e = launch_one<7>(b, pr, hp, keep_windows, out, tl, twin, ovf, device, s); break;
-      default: e = launch_one<8>(b, pr, hp, keep_windows, out, tl, twin, ovf, device, s); break;
+      case 1: e = launch_one<1>(b, pr, hp, keep_windows, out, tl, twin, ovf, s, launches); break;
+      case 2: e = launch_one<2>(b, pr, hp, keep_windows, out, tl, twin, ovf, s, launches); break;
+      case 3: e = launch_one<3>(b, pr, hp, keep_windows, out, tl, twin, ovf, s, launches); break;
+      case 4: e = launch_one<4>(b, pr, hp, keep_windows, out, tl, twin, ovf, s, launches); break;
+      case 5: e = launch_one<5>(b, pr, hp, keep_windows, out, tl, twin, ovf, s, launches); break;
+      case 6: e = launch_one<6>(b, pr, hp, keep_windows, out, tl, twin, ovf, s, launches); break;
+      case 7: e = launch_one<7>(b, pr, hp, keep_windows, out, tl, twin, ovf, s, launches); break;
+      default: e = launch_one<8>(b, pr, hp, keep_windows, out, tl, twin, ovf, s, launches); break;
     }
     if (e != cudaSuccess) return e;
-    ++*n_launches;
   }
   return cudaSuccess;
 }
 
 cudaError_t launch_cut(const tw_batch& b, const tw_score_out& out, const ScoreTiles& st, const int32_t* prev_idx,
-                       cudaStream_t s) {
+                       cudaStream_t s, int64_t& launches) {
   TileList tl{st.tile_prob, st.tile_start, st.n_tiles, kS3Tile};
   k_cut<<<st.n_tiles, kS3Threads, 0, s>>>(b, out, tl, prev_idx, st.overflow);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 }  // namespace tw

@@ -38,9 +38,9 @@ k_skip(tw_batch b, tw_skip_desc sd, tw_skip_out out, uint32_t* __restrict__ take
 
 cudaError_t launch_skip(const tw_batch& b, const tw_skip_desc& sd, const tw_skip_out& out, uint32_t* taken,
                         uint32_t* set_scratch, const int64_t* prob_set_off, int32_t* win_scratch,
-                        long long node_limit, int* err_flag, cudaStream_t s) {
+                        long long node_limit, int* err_flag, cudaStream_t s, int64_t& launches) {
   k_skip<<<b.n_problems, 32, 0, s>>>(b, sd, out, taken, set_scratch, prob_set_off, win_scratch, node_limit, err_flag);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -75,10 +75,10 @@ __global__ void k_build_dist(int n, const int64_t* __restrict__ ms, const int64_
 }
 
 cudaError_t launch_build_dist(int n, const int64_t* ms, const int64_t* me, const int8_t* label, int E,
-                              int64_t large_delay, int32_t* key, int64_t* val, cudaStream_t s) {
+                              int64_t large_delay, int32_t* key, int64_t* val, cudaStream_t s, int64_t& launches) {
   if (n <= 0) return cudaSuccess;
   k_build_dist<<<(n + 127) / 128, 128, 0, s>>>(n, ms, me, label, E, large_delay, key, val);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 }  // namespace tw

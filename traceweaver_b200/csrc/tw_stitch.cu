@@ -953,10 +953,15 @@ extern "C" int tw_debug_stitch_phases(unsigned long long* out16, int reset) {
 }
 #endif
 
+cudaError_t setup_stitch() {
+  return cudaFuncSetAttribute(k_stitch, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)(sizeof(StitchWarpSmem) * kStitchWarps));
+}
+
 cudaError_t launch_stitch(const tw_batch& b, const tw_params& prm, const uint8_t* cut,
                           const tw_score_out& spec, const tw_pass_out& out, uint32_t* taken_words, size_t taken_n_words,
-                          long long node_limit, const StitchUnits& unit_buf, int max_units, int device, int* err_flag,
-                          cudaStream_t s) {
+                          long long node_limit, const StitchUnits& unit_buf, int max_units, int* err_flag,
+                          cudaStream_t s, int64_t& launches) {
   cudaError_t e = cudaMemsetAsync(taken_words, 0, taken_n_words * sizeof(uint32_t), s);
   if (e != cudaSuccess) return e;
   if (out.counters) {
@@ -964,12 +969,6 @@ cudaError_t launch_stitch(const tw_batch& b, const tw_params& prm, const uint8_t
     if (e != cudaSuccess) return e;
   }
   size_t smem = sizeof(StitchWarpSmem) * kStitchWarps;
-  static bool attr_done[64] = {false};
-  if (device >= 0 && device < 64 && !attr_done[device]) {
-    e = cudaFuncSetAttribute(k_stitch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    attr_done[device] = true;
-  }
   StitchUnits units{nullptr, nullptr, nullptr, nullptr};
   int warps = b.n_problems;
   // Units pay when services alone cannot fill the machine (a shipped directory has 2-6 services; the
@@ -981,13 +980,13 @@ cudaError_t launch_stitch(const tw_batch& b, const tw_params& prm, const uint8_t
     e = cudaMemsetAsync(units.count, 0, sizeof(int), s);
     if (e != cudaSuccess) return e;
     k_stitch_units<<<(b.n_problems + 3) / 4, 128, 0, s>>>(b, cut, spec, kStitchUnitMin, units);
-    e = cudaGetLastError();
+    e = after_launch(launches);
     if (e != cudaSuccess) return e;
     warps = max_units;
   }
   int blocks = (warps + kStitchWarps - 1) / kStitchWarps;
   k_stitch<<<blocks, kStitchWarps * 32, smem, s>>>(b, prm, cut, spec, out, taken_words, node_limit, units, err_flag);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 }  // namespace tw

@@ -173,46 +173,52 @@ __global__ void k_in_prob(tw_batch b, int32_t* __restrict__ in_prob) {
   for (int64_t g = a + threadIdx.x; g < z; g += blockDim.x) in_prob[g] = p;
 }
 
-cudaError_t launch_in_prob(const tw_batch& b, int32_t* in_prob, cudaStream_t s) {
+cudaError_t launch_in_prob(const tw_batch& b, int32_t* in_prob, cudaStream_t s, int64_t& launches) {
   k_in_prob<<<b.n_problems, 128, 0, s>>>(b, in_prob);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 cudaError_t launch_ground_truth(const tw_batch& b, const int32_t* in_trace, const int32_t* out_trace,
                                 const int32_t* trace_lo, const int32_t* trace_n, const int64_t* tab_off, int64_t tab_len,
-                                int32_t* tab, const int32_t* in_prob, int32_t* truth, cudaStream_t s) {
+                                int32_t* tab, const int32_t* in_prob, int32_t* truth, cudaStream_t s,
+                                int64_t& launches) {
   cudaError_t e = cudaMemsetAsync(tab, 0x7f, (size_t)tab_len * sizeof(int32_t), s);   // "no position yet"
   if (e != cudaSuccess) return e;
-  if (b.n_out_total > 0)
+  if (b.n_out_total > 0) {
     k_truth_scatter<<<(unsigned)((b.n_out_total + 255) / 256), 256, 0, s>>>(b, out_trace, trace_lo, trace_n, tab_off, tab);
+    e = after_launch(launches);
+    if (e != cudaSuccess) return e;
+  }
   k_truth_gather<<<(unsigned)((b.n_in_total + 255) / 256), 256, 0, s>>>(b, in_trace, trace_lo, trace_n, tab_off, tab, in_prob,
                                                                         truth);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 cudaError_t launch_find_order(const tw_batch& b, const int32_t* truth, const int32_t* in_prob, uint32_t* violated,
-                              int* missing, cudaStream_t s) {
+                              int* missing, cudaStream_t s, int64_t& launches) {
   cudaError_t e = cudaMemsetAsync(violated, 0, (size_t)b.n_ep_total * sizeof(uint32_t), s);
   if (e != cudaSuccess) return e;
   e = cudaMemsetAsync(missing, 0, sizeof(int), s);
   if (e != cudaSuccess) return e;
   k_find_order<<<(unsigned)((b.n_in_total + 255) / 256), 256, 0, s>>>(b, truth, in_prob, violated, missing);
-  return cudaGetLastError();
+  return after_launch(launches);
 }
 
 cudaError_t launch_accuracy(const tw_batch& b, const int32_t* truth, const int32_t* assign, const int32_t* topk_idx,
                             const uint8_t* topk_cnt, const int32_t* in_trace, const int32_t* in_prob,
                             const uint8_t* prob_first, int n_traces, unsigned long long* per_prob, uint8_t* flags,
-                            unsigned long long* trace_first, unsigned long long* out4, cudaStream_t s) {
+                            unsigned long long* trace_first, unsigned long long* out4, cudaStream_t s,
+                            int64_t& launches) {
   uint8_t* seen = flags;
   uint8_t* bad = flags + n_traces;
   uint8_t* kbad = flags + 2 * (size_t)n_traces;
   k_accuracy<<<(unsigned)((b.n_in_total + 255) / 256), 256, 0, s>>>(b, truth, assign, topk_idx, topk_cnt, in_trace, in_prob,
                                                                     prob_first, n_traces, per_prob, seen, bad, trace_first,
                                                                     kbad);
-  if (n_traces > 0)
-    k_accuracy_reduce<<<(n_traces + 255) / 256, 256, 0, s>>>(n_traces, seen, bad, trace_first, kbad, out4);
-  return cudaGetLastError();
+  cudaError_t e = after_launch(launches);
+  if (e != cudaSuccess || n_traces == 0) return e;
+  k_accuracy_reduce<<<(n_traces + 255) / 256, 256, 0, s>>>(n_traces, seen, bad, trace_first, kbad, out4);
+  return after_launch(launches);
 }
 
 }  // namespace tw
