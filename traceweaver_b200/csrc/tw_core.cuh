@@ -606,70 +606,6 @@ TW_HD void enumerate_combos(const ProbView& v, const OutWin* w, const int* lo, c
   }
 }
 
-// One slot of an in-span's term tables, addressed by its local slot index: which term, which
-// candidate(s), their dt — evaluated in place.  This is the body of the slot-parallel pass of the
-// scoring kernel (every thread of the CTA takes slots of ANY in-span of the tile, so the FP64
-// likelihood work is spread evenly).  Returns the slot id (TW_SLOT_INVALID when no feasible tuple
-// can use the slot); *val receives the log-likelihood.  `valid(e, x)`: candidate x of ep e is
-// contained in the in-span and not taken.
-template <class Valid>
-TW_HD uint8_t term_slot_eval(const ProbView& v, const ParamView& pv, int64_t in_s, int64_t in_e, const OutWin* w,
-                             const int* lo, const int* r, int slot, Valid valid, double* val) {
-  int o = 0;
-  for (int e = 0; e < v.E; ++e)
-    for (int t = v.term_lo[e]; t < v.term_lo[e + 1]; ++t) {
-      const int src = v.term_src[t];
-      const int size = src >= 0 ? r[src] * r[e] : r[e];
-      if (slot < o + size) {
-        const int loc = slot - o;
-        int64_t d;
-        bool ok;
-        if (src >= 0) {
-          const int xb = loc / r[e], xe = loc - xb * r[e];
-          const int64_t eb = w[src].e[lo[src] + xb], s = w[e].s[lo[e] + xe];
-          ok = valid(src, xb) && valid(e, xe) && eb <= s;
-          d = s - eb;
-        } else if (src == TW_TERM_ROOT) {
-          ok = valid(e, loc);
-          d = w[e].s[lo[e] + loc] - in_s;
-        } else {
-          ok = valid(e, loc);
-          d = in_e - w[e].e[lo[e] + loc];
-        }
-        if (!ok) return (uint8_t)TW_SLOT_INVALID;
-        *val = term_logpdf(pv, t, (double)d);
-        return (uint8_t)t;
-      }
-      o += size;
-    }
-  return (uint8_t)TW_SLOT_INVALID;
-}
-
-// one combination of the candidate product space (x0-major): feasible tuple?  fills c[] / ce[]
-TW_HD bool combo_feasible(const ProbView& v, const OutWin* w, const int* lo, const int* r, const int* o_last,
-                          const uint8_t* sid, unsigned combo, int* c, int64_t* ce) {
-  int x[TW_MAX_E];
-  int64_t cs[TW_MAX_E];
-  unsigned idx = combo;   // callers keep the product space below 2^31: 32-bit divides
-  bool ok = true;
-  for (int e = v.E - 1; e >= 0; --e) {
-    const unsigned re = (unsigned)r[e], q = idx / re;
-    x[e] = (int)(idx - q * re);
-    idx = q;
-    if (sid[o_last[e] + x[e]] == TW_SLOT_INVALID) ok = false;
-  }
-  if (!ok) return false;
-  for (int e = 0; e < v.E; ++e) {
-    cs[e] = w[e].s[lo[e] + x[e]];
-    ce[e] = w[e].e[lo[e] + x[e]];
-    c[e] = w[e].base + lo[e] + x[e];
-    const uint32_t pm = v.pred[e];
-    for (int b = 0; b < e; ++b)
-      if ((pm >> b & 1u) && ce[b] > cs[e]) return false;
-  }
-  return true;
-}
-
 // order-preserving map double -> uint64 (larger score <=> larger key); NaN maps below -inf
 TW_HD unsigned long long score_key(double s) {
   if (s != s) return 0ULL;

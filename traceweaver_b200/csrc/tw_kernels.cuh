@@ -11,7 +11,7 @@ namespace tw {
 constexpr int kS3Threads = 128;                  // tw_score3.cu: one CTA = one tile, one warp = 32 in-spans
 constexpr int kS3Tile = 128;                     // in-spans per tile
 constexpr int kStageSpans = 1536;                // out spans staged in shared memory per tile
-constexpr int kTblCap = 3072;                    // term-table slots per CTA round (tw_core.cuh)
+constexpr int kTblCap = 3072;                    // term-table slots of a redo CTA (tw_score.cu)
 #ifndef TW_WARP_TBL_CAP
 #define TW_WARP_TBL_CAP 256
 #endif
@@ -49,7 +49,7 @@ struct ScoreTiles {
 // Kernels launched with more than 48 KB of dynamic shared memory need the limit raised once per
 // device: tw_engine_create calls these for the engine's device.
 cudaError_t setup_score3();                      // k_score3<1..TW_MAX_E>
-cudaError_t setup_score();                       // k_score<kWideThreads, kWideW>
+cudaError_t setup_score();                       // k_score
 cudaError_t setup_stitch();                      // k_stitch
 cudaError_t setup_sort_ends();                   // k_sort_ends
 
