@@ -15,7 +15,8 @@
  *     field comment says "host".  `stream` is a cudaStream_t passed as void*.
  *   - every function returns TW_OK (0) or a negative tw_status; nothing throws across the ABI.
  *   - times are int64 microseconds (Jaeger startTime is ~1.7e15 us: differences are formed in
- *     int64 BEFORE conversion to double); scores are IEEE double.
+ *     int64 BEFORE conversion to double); scores are IEEE double.  Fractional (float64) microseconds
+ *     enter through tw_engine_bind_f64, which moves them into exact int64 fixed point.
  *   - "problem" = one service: one incoming endpoint with n_in spans and E outgoing endpoints
  *     ("eps") in the topological order of the invocation graph (traceweaver_v1.py:37-39).
  *     In-spans and each ep's out-spans are sorted by (start, end) (executor.py:1111-1112).
@@ -30,7 +31,7 @@
 extern "C" {
 #endif
 
-#define TW_ABI_VERSION 3
+#define TW_ABI_VERSION 4
 
 /* Algorithm constants hard-coded by the reference. */
 #define TW_MAX_E 8             /* engine limit on out-eps per service (shipped data: <= 4)      */
@@ -171,6 +172,31 @@ int tw_batch_validate_host(const tw_batch* host_desc);
  * The arrays behind `dev` must stay alive and unchanged while bound.
  */
 int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc, void* stream);
+
+/*
+ * Bind a batch whose span times are float64 microseconds (DEVICE arrays, same layout as the tw_batch
+ * span arrays; the span pointers of `dev` are ignored).  This is what executor.py --compress_factor > 1
+ * produces: transforms.repeat_change_spans divides start times by the factor.  Descriptors are validated
+ * as by tw_engine_bind.  Each problem p gets the smallest shift s_p >= 0 such that x * 2^s_p is an
+ * integer for all its start and end times; the engine keeps X = x * 2^s_p in its own int64 buffers.
+ * The conversion is exact and monotone, so windows, cuts, candidate sets and assignments are those of
+ * the float64 times, and every difference the path forms equals the IEEE double difference of the two
+ * times whenever that difference is exact (always inside one binade: Sterbenz).
+ * After this bind the usual sequence (tw_prepare, tw_params_pass0, tw_score_topk, tw_stitch,
+ * tw_delays, tw_gmm_stream_draws, tw_gmm_refit) works unchanged; every parameter, delay and mixture
+ * it takes or returns is in real microseconds.  Pass-0 batch sums are formed exactly and rounded once.
+ * Returns TW_ERR_INVALID for a NaN or infinite time and TW_ERR_RANGE_LIMIT when max|x| * 2^s_p >= 2^55
+ * (headroom for the int64 differences and 100-element sums); tw_last_error() names the problem.
+ * A later tw_engine_bind returns the engine to int64 times.  Blocks until `stream` is idle.
+ */
+typedef struct tw_times_f64 {
+  const double* in_start;        /* [n_in_total]                                                  */
+  const double* in_end;          /* [n_in_total]                                                  */
+  const double* out_start;       /* [n_out_total]                                                 */
+  const double* out_end;         /* [n_out_total]                                                 */
+} tw_times_f64;
+int tw_engine_bind_f64(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc, const tw_times_f64* dev_times,
+                       void* stream);
 
 /*
  * Batch-constant pre-kernels of the path, once per bound batch before the first pass: the

@@ -4,7 +4,7 @@ Field order and widths must match the header exactly; tests/test_abi.py checks s
 against values compiled from the header."""
 import ctypes as C
 
-TW_ABI_VERSION = 3
+TW_ABI_VERSION = 4
 TW_SCORE_KEEP_WINDOWS = 1
 TW_MAX_E = 8
 TW_K = 5
@@ -39,6 +39,10 @@ class TwBatch(C.Structure):
         ("ep_term_off", P), ("ep_pred_mask", P), ("term_src", P),
         ("in_start", P), ("in_end", P), ("out_start", P), ("out_end", P),
     ]
+
+
+class TwTimesF64(C.Structure):
+    _fields_ = [("in_start", P), ("in_end", P), ("out_start", P), ("out_end", P)]
 
 
 class TwParams(C.Structure):

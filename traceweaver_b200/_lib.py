@@ -21,6 +21,8 @@ SYMBOLS = {
     "tw_engine_destroy": (C.c_int, [C.c_void_p]),
     "tw_batch_validate_host": (C.c_int, [C.POINTER(_abi.TwBatch)]),
     "tw_engine_bind": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch), C.c_void_p]),
+    "tw_engine_bind_f64": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch),
+                                     C.POINTER(_abi.TwTimesF64), C.c_void_p]),
     "tw_prepare": (C.c_int, [C.c_void_p, C.c_void_p]),
     "tw_engine_status": (C.c_int, [C.c_void_p, C.c_void_p]),
     "tw_engine_launch_count": (C.c_int64, [C.c_void_p]),

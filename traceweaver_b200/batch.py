@@ -3,11 +3,14 @@
 A *problem* is what the reference hands to `TraceWeaverV3.FindAssignments`
 (executor.py:1172-1175): the spans arriving at one service (one incoming endpoint) and the spans
 it sends to each outgoing endpoint, plus the invocation DAG over the outgoing endpoints.  Here it
-is index-only: int64 microsecond start/end arrays sorted by (start, end) (executor.py:1111-1112),
+is index-only: microsecond start/end arrays sorted by (start, end) (executor.py:1111-1112),
 endpoints in topological order (traceweaver_v1.py:37-39), DAG as predecessor lists in
 `in_edges` order (the order the reference sums likelihood terms in, traceweaver_v1.py:322).
 
 `build_batch` concatenates problems into the arrays of `tw_batch` (include/traceweaver_b200.h).
+Times are int64 microseconds, or float64 microseconds for time-compressed spans (executor.py
+--compress_factor > 1 divides start times by the factor): a batch in which any span array has a
+floating dtype is a float64 batch, and the engine binds it through tw_engine_bind_f64.
 Pure numpy; no device code here.
 """
 from dataclasses import dataclass, field
@@ -17,12 +20,19 @@ import numpy as np
 
 from . import _abi
 
+SPAN_ARRAYS = ("in_start", "in_end", "out_start", "out_end")
+
+
+def _time_dtype(arrays):
+    """float64 if any of the span arrays has a floating dtype, else int64."""
+    return np.float64 if any(np.asarray(a).dtype.kind == "f" for a in arrays) else np.int64
+
 
 @dataclass
 class Problem:
-    in_start: np.ndarray                 # int64 [n_in]
-    in_end: np.ndarray                   # int64 [n_in]
-    out_start: List[np.ndarray]          # per ep (topological order): int64 [n_out_e]
+    in_start: np.ndarray                 # int64 or float64 [n_in]
+    in_end: np.ndarray                   # int64 or float64 [n_in]
+    out_start: List[np.ndarray]          # per ep (topological order): int64 or float64 [n_out_e]
     out_end: List[np.ndarray]
     preds: List[List[int]]               # per ep: predecessor positions, in_edges order
     name: str = ""
@@ -74,7 +84,7 @@ class Problem:
             raise ValueError(f"{self.name}: in_start and in_end differ in length")
         if np.any(self.in_end < self.in_start):
             raise ValueError(f"{self.name}: an in-span ends before it starts")
-        key = self.in_start.astype(np.int64)
+        key = self.in_start if self.in_start.dtype.kind == "f" else self.in_start.astype(np.int64)
         if np.any(np.diff(key) < 0):
             raise ValueError(f"{self.name}: in-spans not sorted by start")
         for e in range(E):
@@ -105,6 +115,11 @@ class HostBatch:
     @property
     def n_problems(self):
         return len(self.problems)
+
+    @property
+    def float_times(self):
+        """True for a batch of float64 microsecond times (bound through tw_engine_bind_f64)."""
+        return self.arrays["in_start"].dtype == np.float64
 
     def no_skip(self):
         """True iff every ep of every problem has n_out == n_in (the regime with two passes,
@@ -167,14 +182,15 @@ def build_batch(problems: Sequence[Problem], validate=True) -> HostBatch:
             mine = [src for (ee, src) in terms if ee == e]
             term_src.extend(mine)
             ep_term_off.append(ep_term_off[-1] + len(mine))
+    tdt = _time_dtype([a for p in problems for a in [p.in_start, p.in_end] + list(p.out_start) + list(p.out_end)])
     arrays = dict(
         prob_in_off=prob_in_off, prob_ep_off=prob_ep_off, prob_tuple_off=prob_tuple_off,
         ep_out_off=np.asarray(ep_out_off, np.int64), ep_term_off=np.asarray(ep_term_off, np.int32),
         ep_pred_mask=np.asarray(ep_pred_mask, np.uint32), term_src=np.asarray(term_src, np.int8),
-        in_start=np.ascontiguousarray(np.concatenate([p.in_start for p in problems]), np.int64),
-        in_end=np.ascontiguousarray(np.concatenate([p.in_end for p in problems]), np.int64),
-        out_start=np.ascontiguousarray(np.concatenate([s for p in problems for s in p.out_start]), np.int64),
-        out_end=np.ascontiguousarray(np.concatenate([s for p in problems for s in p.out_end]), np.int64),
+        in_start=np.ascontiguousarray(np.concatenate([p.in_start for p in problems]), tdt),
+        in_end=np.ascontiguousarray(np.concatenate([p.in_end for p in problems]), tdt),
+        out_start=np.ascontiguousarray(np.concatenate([s for p in problems for s in p.out_start]), tdt),
+        out_end=np.ascontiguousarray(np.concatenate([s for p in problems for s in p.out_end]), tdt),
     )
     n_batches = (np.diff(prob_in_off) + _abi.TW_PARAM_BATCH - 1) // _abi.TW_PARAM_BATCH
     n_terms = np.diff(np.asarray(ep_term_off, np.int64)[prob_ep_off])
@@ -249,15 +265,16 @@ def build_batch_from_blocks(blocks: Sequence[ServiceBlock]) -> HostBatch:
         # per problem: ep 0 list, ep 1 list, ...  -> stack [S, E, n]
         outs.append(np.stack(blk.out_start, axis=1).reshape(-1))
         oute.append(np.stack(blk.out_end, axis=1).reshape(-1))
+    tdt = _time_dtype(ins + ine + outs + oute)
     arrays = dict(
         prob_in_off=np.asarray(prob_in, np.int64), prob_ep_off=np.asarray(prob_ep, np.int32),
         prob_tuple_off=np.asarray(prob_tuple, np.int64), ep_out_off=np.asarray(ep_out, np.int64),
         ep_term_off=np.asarray(ep_term, np.int32), ep_pred_mask=np.asarray(ep_pred, np.uint32),
         term_src=np.asarray(term_src, np.int8),
-        in_start=np.ascontiguousarray(np.concatenate(ins), np.int64),
-        in_end=np.ascontiguousarray(np.concatenate(ine), np.int64),
-        out_start=np.ascontiguousarray(np.concatenate(outs), np.int64),
-        out_end=np.ascontiguousarray(np.concatenate(oute), np.int64))
+        in_start=np.ascontiguousarray(np.concatenate(ins), tdt),
+        in_end=np.ascontiguousarray(np.concatenate(ine), tdt),
+        out_start=np.ascontiguousarray(np.concatenate(outs), tdt),
+        out_end=np.ascontiguousarray(np.concatenate(oute), tdt))
     P = len(prob_in) - 1
     n_in = np.diff(arrays["prob_in_off"])
     n_batches = (n_in + _abi.TW_PARAM_BATCH - 1) // _abi.TW_PARAM_BATCH

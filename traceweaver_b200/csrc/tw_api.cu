@@ -111,6 +111,15 @@ struct tw_engine {
   int n_batches_total = 0;
   DevBuf<int32_t> term_ep;
   DevBuf<int32_t> ep_prob;
+  // float64 timestamps (tw_engine_bind_f64): the fixed-point copies the kernels read, the shift of every
+  // problem, and the scoring copy of the parameter records (k_params_scale)
+  bool shifted = false;
+  DevBuf<int64_t> fixed_times;
+  DevBuf<int32_t> prob_shift;
+  DevBuf<int32_t> prob_top;
+  DevBuf<int32_t> prob_status;
+  DevBuf<double> scaled_params;
+  int64_t n_gauss_rec = 0;
   long long node_limit = 2000000LL;   // exact MWIS search nodes per window before TW_ERR_MWIS_LIMIT
   // refit scratch (allocated on first tw_gmm_refit after bind)
   static constexpr int kStreamLen = 16384;
@@ -225,6 +234,7 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
   if (rc) return rc;
   CU(cudaSetDevice(eng->device));
   eng->bound = false;
+  eng->shifted = false;
   eng->dev = *dev;
   const int P = h->n_problems;
   eng->prob_in_off.assign(h->prob_in_off, h->prob_in_off + P + 1);
@@ -235,6 +245,7 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
   // subdivide scoring tiles and carry their length)
   std::vector<int32_t> nt_prob, nt_start, wt_prob, wt_start, wt_narrow, wt_len, bprob, bidx;
   const int wide_len = kWideThreads - 1;
+  int64_t n_gauss_rec = 0;
   eng->max_seg = 0;
   eng->windows_valid = false;
   eng->class_off[0] = 0;
@@ -262,10 +273,13 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
     if (n > eng->max_seg) eng->max_seg = n;
     int nb = (n + TW_PARAM_BATCH - 1) / TW_PARAM_BATCH;
     for (int q = 0; q < nb; ++q) { bprob.push_back(p); bidx.push_back(q); }
+    const int ep0 = h->prob_ep_off[p];
+    n_gauss_rec += (int64_t)nb * (h->ep_term_off[h->prob_ep_off[p + 1]] - h->ep_term_off[ep0]);
   }
   eng->n_tiles = (int)nt_prob.size();
   eng->n_wide = (int)wt_prob.size();
   eng->n_batches_total = (int)bprob.size();
+  eng->n_gauss_rec = n_gauss_rec;
   std::vector<int32_t> term_ep(h->n_term_total), ep_prob(h->n_ep_total);
   for (int p = 0; p < P; ++p)
     for (int ep = h->prob_ep_off[p]; ep < h->prob_ep_off[p + 1]; ++ep) {
@@ -337,6 +351,63 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
     }
   }
   eng->bound = true;
+  return TW_OK;
+}
+
+int tw_engine_bind_f64(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const tw_times_f64* times,
+                       void* stream_) {
+  if (!eng || !dev || !h || !times || !times->in_start || !times->in_end || !times->out_start || !times->out_end)
+    return fail(TW_ERR_INVALID, "tw_engine_bind_f64: NULL argument");
+  int rc = tw_engine_bind(eng, dev, h, stream_);
+  if (rc) return rc;
+  eng->bound = false;
+  cudaStream_t s = (cudaStream_t)stream_;
+  const int P = h->n_problems;
+  const size_t n_in = (size_t)h->n_in_total, n_out = (size_t)h->n_out_total;
+  CU(eng->fixed_times.reserve(2 * (n_in + n_out)));
+  CU(eng->prob_shift.reserve((size_t)P));
+  CU(eng->prob_top.reserve((size_t)P));
+  CU(eng->prob_status.reserve((size_t)P));
+  CU(cudaMemsetAsync(eng->prob_shift.p, 0, (size_t)P * sizeof(int32_t), s));
+  CU(cudaMemsetAsync(eng->prob_top.p, 0x80, (size_t)P * sizeof(int32_t), s));   // below every floor(log2 |x|)
+  TimesF64 t{times->in_start, times->in_end, times->out_start, times->out_end};
+  CU(launch_to_fixed(eng->dev, t, eng->ep_prob.p, eng->prob_shift.p, eng->prob_top.p, eng->fixed_times.p,
+                     eng->prob_status.p, s, eng->launches));
+  std::vector<int32_t> status((size_t)P);
+  CU(cudaMemcpyAsync(status.data(), eng->prob_status.p, (size_t)P * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  for (int p = 0; p < P; ++p) {
+    if (status[p] == TW_OK) continue;
+    char which[32];
+    snprintf(which, sizeof which, "%d", p);
+    return fail(status[p], status[p] == TW_ERR_INVALID
+                               ? "tw_engine_bind_f64: problem %s has a NaN or infinite timestamp"
+                               : "tw_engine_bind_f64: problem %s needs more than 55 bits in fixed point%s",
+                which, status[p] == TW_ERR_INVALID ? "" : " (magnitude x resolution of its timestamps too large)");
+  }
+  int64_t* fx = eng->fixed_times.p;
+  eng->dev.in_start = fx;
+  eng->dev.in_end = fx + n_in;
+  eng->dev.out_start = fx + 2 * n_in;
+  eng->dev.out_end = fx + 2 * n_in + n_out;
+  eng->shifted = true;
+  eng->bound = true;
+  return TW_OK;
+}
+
+// For a shifted batch the scoring kernels read a rescaled copy of the caller's real-unit records.
+static int scoring_params(tw_engine* eng, const tw_params* params, tw_params& scaled, cudaStream_t s) {
+  scaled = *params;
+  if (!eng->shifted) return TW_OK;
+  const bool gauss = params->mode == TW_PARAMS_GAUSS_BATCHED;
+  const int64_t n_rec = gauss ? eng->n_gauss_rec : eng->dev.n_term_total;
+  const size_t width = gauss ? TW_GAUSS_REC : TW_MIX_REC;
+  CU(eng->scaled_params.reserve((size_t)n_rec * width));
+  CU(launch_params_scale(params->mode, params->prob_gauss_off, eng->dev.n_problems, gauss ? params->gauss : params->mix,
+                         eng->scaled_params.p, n_rec, eng->term_ep.p, eng->ep_prob.p, eng->prob_shift.p, s,
+                         eng->launches));
+  if (gauss) scaled.gauss = eng->scaled_params.p;
+  else scaled.mix = eng->scaled_params.p;
   return TW_OK;
 }
 
@@ -551,7 +622,8 @@ int tw_params_pass0(tw_engine* eng, const int64_t* prob_gauss_off, double* gauss
   int rc = need_bound(eng, "tw_params_pass0");
   if (rc) return rc;
   CU(launch_params0(eng->dev, eng->in_end_sorted.p, eng->out_end_sorted.p, prob_gauss_off, eng->batch_prob.p,
-                    eng->batch_idx.p, eng->n_batches_total, gauss_out, (cudaStream_t)stream, eng->launches));
+                    eng->batch_idx.p, eng->n_batches_total, gauss_out, eng->shifted ? eng->prob_shift.p : nullptr,
+                    (cudaStream_t)stream, eng->launches));
   return TW_OK;
 }
 
@@ -577,6 +649,12 @@ int tw_score_topk(tw_engine* eng, const tw_params* params, const tw_score_out* o
     o.used_lo = eng->own_used_lo.p;
     o.used_bits = eng->own_used_bits.p;
     o.used_wide = eng->own_used_wide.p;
+  }
+  tw_params sp;
+  if (params) {
+    rc = scoring_params(eng, params, sp, s);
+    if (rc) return rc;
+    params = &sp;
   }
   ScoreTiles st;
   st.tile_prob = eng->score_tiles.p;
@@ -614,8 +692,11 @@ int tw_stitch(tw_engine* eng, const tw_params* params, const uint8_t* cut, const
       return fail(TW_ERR_INVALID, "tw_stitch: `undeleted` needs top-K, n_feasible and the used maps");
     spec = *undeleted;
   }
+  tw_params sp;
+  rc = scoring_params(eng, params, sp, (cudaStream_t)stream);
+  if (rc) return rc;
   StitchUnits ub{eng->unit_prob.p, eng->unit_lo.p, eng->unit_hi.p, eng->unit_count.p};
-  CU(launch_stitch(eng->dev, *params, cut, spec, *out, eng->taken.p, eng->taken_words, eng->node_limit, ub,
+  CU(launch_stitch(eng->dev, sp, cut, spec, *out, eng->taken.p, eng->taken_words, eng->node_limit, ub,
                    eng->max_units, eng->err_flag.p, (cudaStream_t)stream, eng->launches));
   return TW_OK;
 }
@@ -625,7 +706,7 @@ int tw_delays(tw_engine* eng, const int32_t* assign, const int64_t* term_sample_
   int rc = need_bound(eng, "tw_delays");
   if (rc) return rc;
   CU(launch_delays(eng->dev, assign, term_sample_off, eng->term_ep.p, eng->ep_prob.p, delays, counts,
-                   (cudaStream_t)stream, eng->launches));
+                   eng->shifted ? eng->prob_shift.p : nullptr, (cudaStream_t)stream, eng->launches));
   return TW_OK;
 }
 

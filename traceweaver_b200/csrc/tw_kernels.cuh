@@ -91,10 +91,29 @@ cudaError_t launch_sort_ends(const tw_batch& b, int64_t* in_end_sorted, int64_t*
 cudaError_t launch_params0(const tw_batch& b, const int64_t* in_end_sorted,
                            const int64_t* out_end_sorted, const int64_t* prob_gauss_off,
                            const int32_t* batch_prob, const int32_t* batch_idx, int n_batches_total,
-                           double* gauss_out, cudaStream_t s, int64_t& launches);
+                           double* gauss_out, const int32_t* prob_shift, cudaStream_t s, int64_t& launches);
 cudaError_t launch_delays(const tw_batch& b, const int32_t* assign, const int64_t* term_sample_off,
                           const int32_t* term_ep, const int32_t* ep_prob, double* delays,
-                          int32_t* counts, cudaStream_t s, int64_t& launches);
+                          int32_t* counts, const int32_t* prob_shift, cudaStream_t s, int64_t& launches);
+
+// ---- float64 timestamps (tw_times.cu): exact fixed point per problem, X = x * 2^shift[p] in int64.
+// prob_shift[p] >= kShiftInvalid marks a problem with a NaN or infinite timestamp.
+constexpr int kShiftInvalid = 1 << 30;
+constexpr int kFixedBits = 55;                   // |X| < 2^55: differences and 100-element sums fit in int64
+struct TimesF64 {
+  const double* in_start;
+  const double* in_end;
+  const double* out_start;
+  const double* out_end;
+};
+// prob_shift / prob_top must be zero / 0x80-byte filled; fx: [in_start | in_end | out_start | out_end] int64;
+// prob_status[p] receives TW_OK, TW_ERR_INVALID (NaN / inf) or TW_ERR_RANGE_LIMIT (|X| >= 2^55).
+cudaError_t launch_to_fixed(const tw_batch& b, const TimesF64& t, const int32_t* ep_prob, int32_t* prob_shift,
+                            int32_t* prob_top, int64_t* fx, int32_t* prob_status, cudaStream_t s, int64_t& launches);
+// scoring copy of real-unit records for a shifted batch (mode of tw_params); n_rec = records of `src`
+cudaError_t launch_params_scale(int mode, const int64_t* prob_gauss_off, int n_problems, const double* src,
+                                double* dst, int64_t n_rec, const int32_t* term_ep, const int32_t* ep_prob,
+                                const int32_t* prob_shift, cudaStream_t s, int64_t& launches);
 
 cudaError_t launch_gmm_prep(int n_terms, const int64_t* term_sample_off, const double* delays,
                             const int32_t* counts, int32_t* max_n, double* mean_var, cudaStream_t s,

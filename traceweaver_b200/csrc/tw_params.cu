@@ -153,10 +153,15 @@ __device__ __forceinline__ double tstd_dev(const double* x, int n) {
   return sqrt(var);
 }
 
+// kShifted: the batch's timestamps are fixed-point values x * 2^prob_shift[p] (tw_engine_bind_f64).  The bin
+// sums stay exact integers; the total and the batch means are taken back to real microseconds (ldexp is
+// exact) before the float tail, so the records, the sigma clamp and log(sigma) are in real units.
+template <bool kShifted>
 __global__ void __launch_bounds__(128)
 k_params0(tw_batch b, const int64_t* __restrict__ in_end_sorted, const int64_t* __restrict__ out_end_sorted,
           const int64_t* __restrict__ prob_gauss_off, const int32_t* __restrict__ batch_prob,
-          const int32_t* __restrict__ batch_idx, int n_batches_total, double* __restrict__ gauss_out) {
+          const int32_t* __restrict__ batch_idx, int n_batches_total, double* __restrict__ gauss_out,
+          const int32_t* __restrict__ prob_shift) {
   const int wid = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
   if (wid >= n_batches_total) return;
@@ -200,9 +205,14 @@ k_params0(tw_batch b, const int64_t* __restrict__ in_end_sorted, const int64_t* 
         for (int q = 0; q < TW_PARAM_NBATCHES; ++q) {
           tot += bin[q];
           int a0 = q * bs, z0 = min(m, (q + 1) * bs);
-          if (z0 - a0 > 0) bm[nb++] = ddiv((double)bin[q], (double)(z0 - a0));
+          if (z0 - a0 > 0) {
+            if constexpr (kShifted) bm[nb++] = ddiv(ldexp((double)bin[q], -prob_shift[p]), (double)(z0 - a0));
+            else bm[nb++] = ddiv((double)bin[q], (double)(z0 - a0));
+          }
         }
-        double mean = ddiv((double)tot, (double)m);
+        double mean;
+        if constexpr (kShifted) mean = ddiv(ldexp((double)tot, -prob_shift[p]), (double)m);
+        else mean = ddiv((double)tot, (double)m);
         double sd = dmul(sqrt((double)bs), tstd_dev(bm, nb));
         if (sd < 1.0e-12) sd = 0.001;                                   // V1:130-131
         double* rec = gauss_out + (prob_gauss_off[p] + (int64_t)bt * n_terms + t) * TW_GAUSS_REC;
@@ -214,10 +224,15 @@ k_params0(tw_batch b, const int64_t* __restrict__ in_end_sorted, const int64_t* 
 
 cudaError_t launch_params0(const tw_batch& b, const int64_t* in_end_sorted, const int64_t* out_end_sorted,
                            const int64_t* prob_gauss_off, const int32_t* batch_prob, const int32_t* batch_idx,
-                           int n_batches_total, double* gauss_out, cudaStream_t s, int64_t& launches) {
+                           int n_batches_total, double* gauss_out, const int32_t* prob_shift, cudaStream_t s,
+                           int64_t& launches) {
   int blocks = (n_batches_total + 3) / 4;
-  k_params0<<<blocks, 128, 0, s>>>(b, in_end_sorted, out_end_sorted, prob_gauss_off, batch_prob, batch_idx,
-                                   n_batches_total, gauss_out);
+  if (prob_shift)
+    k_params0<true><<<blocks, 128, 0, s>>>(b, in_end_sorted, out_end_sorted, prob_gauss_off, batch_prob, batch_idx,
+                                           n_batches_total, gauss_out, prob_shift);
+  else
+    k_params0<false><<<blocks, 128, 0, s>>>(b, in_end_sorted, out_end_sorted, prob_gauss_off, batch_prob, batch_idx,
+                                            n_batches_total, gauss_out, nullptr);
   return after_launch(launches);
 }
 
@@ -225,10 +240,13 @@ cudaError_t launch_params0(const tw_batch& b, const int64_t* in_end_sorted, cons
 // Delay samples per term from a pass's assignments (V3:721-760).  One warp per term, ballot
 // compaction keeps in-span order (the refit's k-means++ seeding indexes samples by position).
 // ---------------------------------------------------------------------------------------------
+// kShifted: fixed-point timestamps (see k_params0); the exact integer difference is converted, then scaled
+// back to real microseconds by ldexp, which is exact.
+template <bool kShifted>
 __global__ void __launch_bounds__(128)
 k_delays(tw_batch b, const int32_t* __restrict__ assign, const int64_t* __restrict__ term_sample_off,
          const int32_t* __restrict__ term_ep, const int32_t* __restrict__ ep_prob,
-         double* __restrict__ delays, int32_t* __restrict__ counts) {
+         double* __restrict__ delays, int32_t* __restrict__ counts, const int32_t* __restrict__ prob_shift) {
   const int t = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
   if (t >= b.n_term_total) return;
@@ -261,6 +279,7 @@ k_delays(tw_batch b, const int32_t* __restrict__ assign, const int64_t* __restri
         else { ok = true; d = (double)(b.in_end[in_off + i] - oe_e[ce]); }
       }
     }
+    if constexpr (kShifted) d = ldexp(d, -prob_shift[p]);
     unsigned mask = __ballot_sync(0xffffffffu, ok);
     if (ok) dst[base + __popc(mask & ((1u << lane) - 1u))] = d;
     base += __popc(mask);
@@ -270,9 +289,12 @@ k_delays(tw_batch b, const int32_t* __restrict__ assign, const int64_t* __restri
 
 cudaError_t launch_delays(const tw_batch& b, const int32_t* assign, const int64_t* term_sample_off,
                           const int32_t* term_ep, const int32_t* ep_prob, double* delays, int32_t* counts,
-                          cudaStream_t s, int64_t& launches) {
+                          const int32_t* prob_shift, cudaStream_t s, int64_t& launches) {
   int blocks = (b.n_term_total + 3) / 4;
-  k_delays<<<blocks, 128, 0, s>>>(b, assign, term_sample_off, term_ep, ep_prob, delays, counts);
+  if (prob_shift)
+    k_delays<true><<<blocks, 128, 0, s>>>(b, assign, term_sample_off, term_ep, ep_prob, delays, counts, prob_shift);
+  else
+    k_delays<false><<<blocks, 128, 0, s>>>(b, assign, term_sample_off, term_ep, ep_prob, delays, counts, nullptr);
   return after_launch(launches);
 }
 

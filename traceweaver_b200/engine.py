@@ -6,7 +6,7 @@ import numpy as np
 import torch
 
 from . import _abi, _lib
-from .batch import HostBatch, batch_struct
+from .batch import SPAN_ARRAYS, HostBatch, batch_struct
 
 
 def _to_device(a: np.ndarray, device, pinned=False):
@@ -72,20 +72,25 @@ class Engine:
     # -- binding ---------------------------------------------------------------------------------
     def bind(self, hb: HostBatch, device_arrays=None, pinned=False):
         """Upload (or adopt) the batch arrays and bind them.  `device_arrays`: dict of tensors
-        already resident on the device for the four span arrays."""
+        already resident on the device for the four span arrays.  A batch with float64 span arrays
+        (fractional microseconds) is bound through tw_engine_bind_f64."""
         self.hb = hb
         d = {}
         for name, a in hb.arrays.items():
             if device_arrays and name in device_arrays:
                 d[name] = device_arrays[name]
             else:
-                d[name] = _to_device(a, self.device, pinned=pinned and name in (
-                    "in_start", "in_end", "out_start", "out_end"))
+                d[name] = _to_device(a, self.device, pinned=pinned and name in SPAN_ARRAYS)
         self.d = d
         self.dev_struct = batch_struct(hb, lambda n: d[n].data_ptr())
         self.host_struct = batch_struct(hb, lambda n: hb.arrays[n].ctypes.data)
-        _lib.check(self.lib.tw_engine_bind(self.h, C.byref(self.dev_struct), C.byref(self.host_struct),
-                                           self.stream), "tw_engine_bind")
+        if hb.float_times:
+            self.times_struct = _abi.TwTimesF64(*[d[n].data_ptr() for n in SPAN_ARRAYS])
+            _lib.check(self.lib.tw_engine_bind_f64(self.h, C.byref(self.dev_struct), C.byref(self.host_struct),
+                                                   C.byref(self.times_struct), self.stream), "tw_engine_bind_f64")
+        else:
+            _lib.check(self.lib.tw_engine_bind(self.h, C.byref(self.dev_struct), C.byref(self.host_struct),
+                                               self.stream), "tw_engine_bind")
         self.n_in = int(hb.prob_in_off[-1])
         self.n_tuple = int(hb.prob_tuple_off[-1])
         return self

@@ -76,17 +76,24 @@ class TraceWeaverV3:
         self.skip_state = skipmode.SkipState()
         self.carry_state = carry_state
         self._pending_dist = []
+        self._fractional_state = False        # parked skip-regime state came from a service with float times
 
     # -- marshalling -------------------------------------------------------------------------------
     @staticmethod
-    def _arrays(spans):
-        raw = [sp.start_mus for sp in spans]
-        if any(isinstance(x, float) and x != int(x) for x in raw):
-            # executor.py --compress_factor > 1 (transforms.repeat_change_spans) divides the start times: float
-            # microseconds, which the engine's int64 timestamps cannot hold — loud, not truncated
-            raise NotImplementedError("fractional start_mus (time-compressed spans): outside the engine's int64 "
-                                      "timestamp model; use the reference for --compress_factor > 1")
-        s = np.fromiter((int(x) for x in raw), np.int64, len(spans))
+    def _fractional(spans):
+        return any(isinstance(sp.start_mus, float) and sp.start_mus != int(sp.start_mus) for sp in spans)
+
+    @staticmethod
+    def _arrays(spans, fractional=False):
+        """(start, end) arrays.  fractional: float64 microseconds — executor.py --compress_factor > 1
+        (transforms.repeat_change_spans) divides the start times — with end = start_mus + duration_mus
+        formed in Python float arithmetic as the reference does; the engine solves them in exact fixed
+        point (tw_engine_bind_f64)."""
+        if fractional:
+            s = np.fromiter((float(sp.start_mus) for sp in spans), np.float64, len(spans))
+            e = np.fromiter((float(sp.start_mus) + sp.duration_mus for sp in spans), np.float64, len(spans))
+            return s, e
+        s = np.fromiter((int(sp.start_mus) for sp in spans), np.int64, len(spans))
         d = np.fromiter((sp.duration_mus for sp in spans), np.int64, len(spans))
         return s, s + d
 
@@ -96,8 +103,9 @@ class TraceWeaverV3:
         if set(out_eps) != set(out_span_partitions.keys()):
             raise ValueError("invocation_graph nodes must be the outgoing endpoints")
         pos = {ep: i for i, ep in enumerate(out_eps)}
-        in_s, in_e = self._arrays(in_spans)
-        outs = [self._arrays(out_span_partitions[ep]) for ep in out_eps]
+        frac = self._fractional(in_spans) or any(self._fractional(p) for p in out_span_partitions.values())
+        in_s, in_e = self._arrays(in_spans, frac)
+        outs = [self._arrays(out_span_partitions[ep], frac) for ep in out_eps]
         preds = [[pos[b] for b, _ in invocation_graph.in_edges(ep)] for ep in out_eps]
         prob = Problem(in_start=in_s, in_end=in_e, out_start=[o[0] for o in outs], out_end=[o[1] for o in outs],
                        preds=preds, name=process)
@@ -117,6 +125,13 @@ class TraceWeaverV3:
         in_spans = sorted(in_spans, key=lambda x: float(x.start_mus))
         if any(len(p) != len(in_spans) for p in out_span_partitions.values()):
             # skip budgets (cache hits / dynamism): ONE iteration with skip spans, traceweaver_v3.py:1138-1158
+            if self._fractional(in_spans) or any(self._fractional(p) for p in out_span_partitions.values()):
+                raise NotImplementedError("fractional start_mus (time-compressed spans) on a service with skip "
+                                          "budgets: the skip regime keeps int64 timestamps; use the reference")
+            if self.carry_state and self._fractional_state:
+                raise NotImplementedError("a service with skip budgets after a service with fractional start_mus: "
+                                          "the skip regime would read state built from fractional timestamps; "
+                                          "use carry_state=False or the reference")
             return self._find_assignments_skip(process, in_ep, in_spans, out_span_partitions, true_assignments,
                                                invocation_graph)
         out_parts = {ep: sorted(p, key=lambda x: float(x.start_mus)) for ep, p in out_span_partitions.items()}
@@ -141,6 +156,7 @@ class TraceWeaverV3:
             # windows are appended now (a few tuples), the distribution samples are derived lazily — the
             # arrays are parked and run through tw_build_dist_samples, in call order, when a service with
             # skip budgets actually arrives (_find_assignments_skip)
+            self._fractional_state |= hb.float_times
             self.skip_state.time_windows.extend(skipmode.new_time_windows(prob.in_start, prob.in_end))
             self._pending_dist.append((prob.in_start, prob.in_end, prob.out_start, prob.out_end, [in_ep] + out_eps))
         dev = self.engine.device
