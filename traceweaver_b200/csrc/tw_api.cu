@@ -100,6 +100,8 @@ struct tw_engine {
   DevBuf<int32_t> unit_hi;
   DevBuf<int> unit_count;
   int max_units = 0;
+  StitchLayout stitch_layout{};      // per-warp shared memory of k_stitch for the bound batch
+  DevBuf<StitchTables> stitch_tables;   // search tables, one per stitch warp
   DevBuf<int32_t> long_seg;          // lists longer than kSortSmemCap (sorted in global memory)
   int n_long = 0;
   DevBuf<int64_t> long_scratch;
@@ -325,6 +327,19 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
     CU(eng->unit_lo.reserve((size_t)mu));
     CU(eng->unit_hi.reserve((size_t)mu));
     CU(eng->unit_count.reserve(1));
+  }
+  // shared-memory slab of a stitch warp: sized for the batch's largest E and largest taken bitmap
+  {
+    int e_max = 1, tk_max = 0;
+    for (int p = 0; p < P; ++p) {
+      const int ep0 = h->prob_ep_off[p], E = h->prob_ep_off[p + 1] - ep0;
+      int tk = 0;
+      for (int e = 0; e < E; ++e) tk += (int)((h->ep_out_off[ep0 + e + 1] - h->ep_out_off[ep0 + e]) >> 5) + 3;
+      e_max = E > e_max ? E : e_max;
+      tk_max = tk > tk_max ? tk : tk_max;
+    }
+    eng->stitch_layout = stitch_layout(e_max, tk_max);
+    CU(eng->stitch_tables.reserve((size_t)(P > eng->max_units ? P : eng->max_units) + kStitchWarps));
   }
   // lists too long for the shared-memory sort of tw_prepare get a slab of global scratch each
   {
@@ -697,7 +712,8 @@ int tw_stitch(tw_engine* eng, const tw_params* params, const uint8_t* cut, const
   if (rc) return rc;
   StitchUnits ub{eng->unit_prob.p, eng->unit_lo.p, eng->unit_hi.p, eng->unit_count.p};
   CU(launch_stitch(eng->dev, sp, cut, spec, *out, eng->taken.p, eng->taken_words, eng->node_limit, ub,
-                   eng->max_units, eng->err_flag.p, (cudaStream_t)stream, eng->launches));
+                   eng->max_units, eng->stitch_layout, eng->stitch_tables.p, eng->err_flag.p, (cudaStream_t)stream,
+                   eng->launches));
   return TW_OK;
 }
 

@@ -692,12 +692,32 @@ TW_HD bool bitmaps_intersect(const uint32_t* A, int loA, const uint32_t* B, int 
 // none"), after splitting the window into connected components of the in-span conflict graph.
 // Vertices with weight <= 0 are never taken (score < -10000, SURVEY A.9 item 6).
 // ---------------------------------------------------------------------------------------------
+// The window functions below take either buffer type; they reach tuple position e of candidate
+// (in-span k, rank r) only through at(k, r, e).
 struct WindowBuf {
   double score[TW_WINDOW_CAP][TW_K];
   int idx[TW_WINDOW_CAP][TW_K][TW_MAX_E];
   int cnt[TW_WINDOW_CAP];
   int chosen[TW_WINDOW_CAP];
   uint32_t adj[TW_WINDOW_CAP];
+  TW_HD int& at(int k, int r, int e) { return idx[k][r][e]; }
+  TW_HD int at(int k, int r, int e) const { return idx[k][r][e]; }
+};
+
+// The window buffer of the stitch kernel: one plane of candidates per tuple position, the last member,
+// so a holder may provide only packed_bytes(E_max) bytes, the planes of its largest E (the stitch
+// kernel's per-warp slab, sized per batch).  Lane 5k + r reading (k, r) hits 32 distinct banks.
+struct PackedWindowBuf {
+  double score[TW_WINDOW_CAP][TW_K];
+  int cnt[TW_WINDOW_CAP];
+  int chosen[TW_WINDOW_CAP];
+  uint32_t adj[TW_WINDOW_CAP];
+  int idx[TW_MAX_E][TW_WINDOW_CAP * TW_K];
+  TW_HD int& at(int k, int r, int e) { return idx[e][k * TW_K + r]; }
+  TW_HD int at(int k, int r, int e) const { return idx[e][k * TW_K + r]; }
+  static constexpr int packed_bytes(int e_max) {
+    return (int)(sizeof(PackedWindowBuf) - sizeof(int) * TW_WINDOW_CAP * TW_K * (TW_MAX_E - e_max));
+  }
 };
 
 TW_HD bool tuples_conflict(const int* a, const int* b, int E) {
@@ -706,15 +726,24 @@ TW_HD bool tuples_conflict(const int* a, const int* b, int E) {
   return false;
 }
 
+// candidates (k, r) and (a, q) of a window share an out span at some tuple position
+template <class WB>
+TW_HD bool cands_conflict(const WB& wb, int k, int r, int a, int q, int E) {
+  for (int e = 0; e < E; ++e)
+    if (wb.at(k, r, e) == wb.at(a, q, e)) return true;
+  return false;
+}
+
 // in-span level adjacency: bit a of adj[k] <=> some candidate of k conflicts with some of a
-TW_HD uint32_t window_adjacency(const WindowBuf& wb, int E, int nw, int k) {
+template <class WB>
+TW_HD uint32_t window_adjacency(const WB& wb, int E, int nw, int k) {
   uint32_t m = 0;
   for (int a = 0; a < nw; ++a) {
     if (a == k) continue;
     bool hit = false;
     for (int r = 0; r < wb.cnt[k] && !hit; ++r)
       for (int q = 0; q < wb.cnt[a] && !hit; ++q)
-        hit = tuples_conflict(wb.idx[k][r], wb.idx[a][q], E);
+        hit = cands_conflict(wb, k, r, a, q, E);
     if (hit) m |= 1u << a;
   }
   return m;
@@ -734,7 +763,8 @@ constexpr int kMwisSimpleBudget = 1024;   // nodes the plain search may spend on
 // below).  best != nullptr: the matching (first tied optimum); price != nullptr: the dual price of
 // every candidate's column and their total (a candidate's weight never exceeds its row's dual plus
 // its column's price; prices are >= 0).
-TW_HD_NOINLINE inline void assignment_solve(const WindowBuf& wb, const int* member, int m, int pos, int* best,
+template <class WB>
+TW_HD_NOINLINE inline void assignment_solve(const WB& wb, const int* member, int m, int pos, int* best,
                                             double (*price)[TW_K], double* price_total) {
   // columns 1..ncol: distinct out spans; ncol+1..ncol+m: "row l stays unassigned"
   int colid[TW_WINDOW_CAP * TW_K];
@@ -745,7 +775,7 @@ TW_HD_NOINLINE inline void assignment_solve(const WindowBuf& wb, const int* memb
     for (int r = 0; r < TW_K; ++r) {
       ecol[l][r] = -1;
       if (r >= wb.cnt[k] || !(TW_WEIGHT_OFFSET + wb.score[k][r] > 0.0)) continue;
-      const int span = wb.idx[k][r][pos];
+      const int span = wb.at(k, r, pos);
       int j = 0;
       while (j < ncol && colid[j] != span) ++j;
       if (j == ncol) colid[ncol++] = span;
@@ -896,7 +926,8 @@ TW_HD_NOINLINE inline void assignment_solve(const WindowBuf& wb, const int* memb
 // here but returned as in-span masks (up to TW_MWIS_MAX_DEFERRED; *n_deferred counts them) for the
 // caller's warp-wide priced search (tw_stitch.cu); nullptr: everything is solved here.
 #define TW_MWIS_MAX_DEFERRED 4
-TW_HD_NOINLINE inline long long mwis_solve(WindowBuf& wb, int E, int nw, long long node_limit,
+template <class WB>
+TW_HD_NOINLINE inline long long mwis_solve(WB& wb, int E, int nw, long long node_limit,
                                            uint32_t* deferred = nullptr, int* n_deferred = nullptr) {
   long long nodes = 0;
   if (n_deferred) *n_deferred = 0;
@@ -989,7 +1020,7 @@ TW_HD_NOINLINE inline long long mwis_solve(WindowBuf& wb, int E, int nw, long lo
         bool ok = true;
         for (int l = 0; l < level && ok; ++l)
           if (choice[l] >= 0 && (wb.adj[k] >> member[l] & 1u) &&
-              tuples_conflict(wb.idx[k][r], wb.idx[member[l]][choice[l]], E))
+              cands_conflict(wb, k, r, member[l], choice[l], E))
             ok = false;
         if (!ok) continue;
         choice[level] = r;
@@ -1035,11 +1066,11 @@ TW_HD_NOINLINE inline long long mwis_solve(WindowBuf& wb, int E, int nw, long lo
         int distinct = 0;
         for (int l = 0; l < m; ++l)
           for (int r = 0; r < wb.cnt[member[l]]; ++r) {
-            const int sp = wb.idx[member[l]][r][e];
+            const int sp = wb.at(member[l], r, e);
             bool seen = false;
             for (int l2 = 0; l2 <= l && !seen; ++l2)
               for (int r2 = 0; r2 < (l2 < l ? wb.cnt[member[l2]] : r) && !seen; ++r2)
-                seen = wb.idx[member[l2]][r2][e] == sp;
+                seen = wb.at(member[l2], r2, e) == sp;
             distinct += !seen;
           }
         if (distinct < fewest) { fewest = distinct; pos = e; }
@@ -1130,7 +1161,7 @@ TW_HD_NOINLINE inline long long mwis_solve(WindowBuf& wb, int E, int nw, long lo
         if (mask && (wb.adj[k] >> member[j] & 1u)) {
           const int kj = member[j];
           for (int q = 0; q < wb.cnt[kj]; ++q)
-            if ((mask >> q & 1u) && tuples_conflict(wb.idx[k][r], wb.idx[kj][q], E)) mask &= (uint8_t)~(1u << q);
+            if ((mask >> q & 1u) && cands_conflict(wb, k, r, kj, q, E)) mask &= (uint8_t)~(1u << q);
         }
         avail[level + 1][j] = mask;
         rest += best_avail(j, mask);

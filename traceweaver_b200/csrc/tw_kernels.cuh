@@ -25,6 +25,28 @@ constexpr int kWideThreads = 32;                 // (31 in-spans + carry-in per 
 
 // ---- stitch kernel geometry (tw_stitch.cu) --------------------------------------------------
 constexpr int kStitchWarps = 2;                  // one warp per problem
+// Register budget of k_stitch: 14 CTAs = 28 resident warps per SM at 72 registers.  A 64-register
+// budget (32 warps) spills in the hot loop and measured slower on an H100.
+constexpr int kStitchBlocksPerSM = 14;
+
+// Term tables of the search tier (and price scratch of the warp-wide MWIS) of one stitch warp: in
+// global memory, one per launched warp, so that shared memory holds only what every window touches.
+struct StitchTables {
+  double tbl[kWarpTblCap];
+  uint8_t sid[kWarpTblCap];
+};
+
+// Per-warp shared-memory slab of k_stitch, sized per bound batch (stitch_layout): the fixed part
+// (problem view, small-window solver scratch), the taken bitmap and its scratch copy sized for the
+// batch's largest service (at most kTakenWords words; larger services use global memory), and the
+// window buffer with the tuple planes of the batch's largest E.
+struct StitchLayout {
+  int tk_words;                                  // words of the taken bitmap (and of its scratch copy)
+  int wb_off;                                    // byte offset of the PackedWindowBuf
+  int bytes;                                     // slab bytes per warp
+};
+// e_max / tk_words_max: largest E and largest taken bitmap (sum over eps of n_out / 32 + 3) of the batch
+StitchLayout stitch_layout(int e_max, int tk_words_max);
 
 // Tiles: a tile never crosses a problem.  tile_prob[t], tile_start[t] (problem-local in-span).
 struct TileList {
@@ -80,10 +102,11 @@ struct StitchUnits {
 };
 constexpr int kStitchUnitMin = 48;               // a unit is closed at the first strong cut after this many in-spans
 constexpr int kStitchUnitMaxServices = 4096;     // batches with at least this many services keep one warp per service
+// `tables`: one StitchTables per launched warp (max(n_problems, max_units) + kStitchWarps)
 cudaError_t launch_stitch(const tw_batch& b, const tw_params& prm, const uint8_t* cut,
                           const tw_score_out& spec, const tw_pass_out& out, uint32_t* taken_words, size_t taken_n_words,
-                          long long node_limit, const StitchUnits& unit_buf, int max_units, int* err_flag,
-                          cudaStream_t s, int64_t& launches);
+                          long long node_limit, const StitchUnits& unit_buf, int max_units, const StitchLayout& layout,
+                          StitchTables* tables, int* err_flag, cudaStream_t s, int64_t& launches);
 constexpr int kSortSmemCap = 16384;               // longest list the shared-memory sort network takes
 cudaError_t launch_sort_ends(const tw_batch& b, int64_t* in_end_sorted, int64_t* out_end_sorted,
                              int max_seg, const int32_t* long_seg, int n_long, int64_t* long_scratch,

@@ -38,15 +38,25 @@ __device__ __forceinline__ void prefetch_l1(const void* p) {
   asm volatile("prefetch.global.L1 [%0];" ::"l"(p));
 }
 
+// Fixed part of a warp's slab; the rest is laid out per batch (StitchLayout, stitch_layout):
+//   uint32_t tk[tk_words]     taken bitmap of the service when it fits (else global memory)
+//   uint32_t tmp[tk_words]    scratch bitmap of the run path (always left zero)
+//   PackedWindowBuf           at wb_off, the tuple planes of the batch's largest E
 struct StitchWarpSmem {
   ProbView v;
-  WindowBuf wb;
-  double tbl[kWarpTblCap];     // term tables of the current window (tw_core.cuh)
-  uint32_t tk[kTakenWords];    // taken bitmap of the service when it fits (else global memory)
-  uint32_t tmp[kTakenWords];   // scratch bitmap of the run path (always left zero)
-  uint8_t sid[kWarpTblCap];
   uint32_t cconf[32];          // small-window solver: conflict mask / weight of candidate lane 5k + r
   double cw[32];
+};
+static_assert(sizeof(StitchWarpSmem) % 8 == 0, "the taken bitmaps and the window buffer follow 8-byte aligned");
+
+// The slab of one warp and the pointers into it; every access to the per-batch part goes through here.
+struct StitchSlab {
+  unsigned char* base;
+  __device__ StitchWarpSmem& fixed() const { return *reinterpret_cast<StitchWarpSmem*>(base); }
+  __device__ uint32_t* taken() const { return reinterpret_cast<uint32_t*>(base + sizeof(StitchWarpSmem)); }
+  __device__ PackedWindowBuf& window(const StitchLayout& L) const {
+    return *reinterpret_cast<PackedWindowBuf*>(base + L.wb_off);
+  }
 };
 
 // Exact MWIS of a window of <= 6 in-spans by the whole warp.  Candidate (in-span k, rank r) lives in
@@ -61,15 +71,15 @@ struct StitchWarpSmem {
 // sequential solver: E == 1 with >= 3 in-spans (Hungarian path) or more than kSmallSpace leaves.
 constexpr int kSmallWindow = 6;
 constexpr int kSmallSpace = 4096;
-__device__ __forceinline__ bool stitch_small_window(StitchWarpSmem& sm, int E, int nw, int lane, long long* nodes_out) {
-  WindowBuf& wb = sm.wb;
+__device__ __forceinline__ bool stitch_small_window(StitchWarpSmem& sm, PackedWindowBuf& wb, int E, int nw, int lane,
+                                                    long long* nodes_out) {
   const unsigned kAll = 0xffffffffu;
   const int k = lane / TW_K, r = lane - TW_K * k;
   const bool valid = k < nw && r < wb.cnt[k];
   const unsigned vmask = __ballot_sync(kAll, valid);
   uint32_t conf = 0u;
   if (valid) {
-    for (int e = 0; e < E; ++e) conf |= __match_any_sync(vmask, wb.idx[k][r][e]);
+    for (int e = 0; e < E; ++e) conf |= __match_any_sync(vmask, wb.at(k, r, e));
     conf &= ~(0x1fu << (TW_K * k));
   }
   sm.cconf[lane] = conf;
@@ -183,8 +193,8 @@ __device__ __forceinline__ bool stitch_small_window(StitchWarpSmem& sm, int E, i
 // expanded by all lanes at once — the owner's choice is broadcast, every later in-span strikes its
 // conflicting ranks, two warp sums give the bounds of the child — so a node costs tens of
 // instructions instead of the hundreds of the one-lane loop over (in-span, rank, tuple position).
-// `price` (shared scratch): dual prices of one callee's assignment relaxation, written by lane 0.
-__device__ __noinline__ long long mwis_component_warp(WindowBuf& wb, int E, uint32_t comp, double* price /*[31][TW_K]*/,
+// `price` (the warp's StitchTables): dual prices of one callee's assignment relaxation, written by lane 0.
+__device__ __noinline__ long long mwis_component_warp(PackedWindowBuf& wb, int E, uint32_t comp, double* price /*[31][TW_K]*/,
                                                       long long node_limit, long long nodes, int lane) {
   const unsigned kAll = 0xffffffffu;
   // members in window order
@@ -211,11 +221,11 @@ __device__ __noinline__ long long mwis_component_warp(WindowBuf& wb, int E, uint
       int distinct = 0;
       for (int l = 0; l < m; ++l)
         for (int r = 0; r < wb.cnt[member[l]]; ++r) {
-          const int sp = wb.idx[member[l]][r][e];
+          const int sp = wb.at(member[l], r, e);
           bool seen = false;
           for (int l2 = 0; l2 <= l && !seen; ++l2)
             for (int r2 = 0; r2 < (l2 < l ? wb.cnt[member[l2]] : r) && !seen; ++r2)
-              seen = wb.idx[member[l2]][r2][e] == sp;
+              seen = wb.at(member[l2], r2, e) == sp;
           distinct += !seen;
         }
       if (distinct < fewest) { fewest = distinct; pos = e; }
@@ -308,7 +318,7 @@ __device__ __noinline__ long long mwis_component_warp(WindowBuf& wb, int E, uint
     uint8_t mask = avmine;
     if (mine && lane > level && mask && (wb.adj[kL] >> kmine & 1u)) {
       for (int q = 0; q < cnt; ++q)
-        if ((mask >> q & 1u) && tuples_conflict(wb.idx[kL][r], wb.idx[kmine][q], E)) mask &= (uint8_t)~(1u << q);
+        if ((mask >> q & 1u) && cands_conflict(wb, kL, r, kmine, q, E)) mask &= (uint8_t)~(1u << q);
     }
     av[level + 1] = mask;
     const bool later = mine && lane > level;
@@ -328,16 +338,15 @@ __device__ __noinline__ long long mwis_component_warp(WindowBuf& wb, int E, uint
 }
 
 // Search path of one window: the lanes flagged `todo` enumerate + score their in-span on the
-// not-yet-taken out spans (term tables in the warp's shared memory, evaluated by all lanes) and leave
+// not-yet-taken out spans (term tables in the warp's StitchTables, evaluated by all lanes) and leave
 // their top-K lists in the window buffer.  Out of line on purpose: it is large and rarely taken (an
 // in-span gets here only when one of its candidates was taken by an earlier window).
-__device__ __noinline__ void stitch_search_lanes(StitchWarpSmem& sm, const tw_params& prm, const tw_pass_out& out,
+__device__ __noinline__ void stitch_search_lanes(const ProbView& v, PackedWindowBuf& wb, StitchTables& tb,
+                                                 const tw_params& prm, const tw_pass_out& out,
                                                  uint32_t* const* tk_base, const OutWin* w,
                                                  const double* gauss_base, const double* mix_base, const double* etab,
                                                  int E, int lane, int ws, int i, int64_t in_s, int64_t in_e,
                                                  bool todo, int batch0) {
-  const ProbView& v = sm.v;
-  WindowBuf& wb = sm.wb;
   auto is_taken = [&](int e, int o) {   // volatile: bits are set by other lanes with atomics
     return (reinterpret_cast<volatile const uint32_t*>(tk_base[e])[o >> 5] >> (o & 31)) & 1u;
   };
@@ -359,7 +368,7 @@ __device__ __noinline__ void stitch_search_lanes(StitchWarpSmem& sm, const tw_pa
     wb.cnt[lane] = tk.n;
     for (int k = 0; k < tk.n; ++k) {
       wb.score[lane][k] = tk.score[k];
-      for (int e = 0; e < E; ++e) wb.idx[lane][k][e] = tk.idx[k][e];
+      for (int e = 0; e < E; ++e) wb.at(lane, k, e) = tk.idx[k][e];
     }
     if (out.topk_score) {
       out.topk_cnt[gi] = (uint8_t)tk.n;
@@ -392,17 +401,17 @@ __device__ __noinline__ void stitch_search_lanes(StitchWarpSmem& sm, const tw_pa
       const int brel_b = __shfl_sync(0xffffffffu, brel, L);
       const long long P_b = __shfl_sync(0xffffffffu, Pown, L);
       term_table_last_offsets(v, r_b, o_last_b);
-      if (lane == L) term_table_fill(v, in_s, in_e, w, lo, r, o_last_b, brel_b, is_taken, sm.tbl, sm.sid);
+      if (lane == L) term_table_fill(v, in_s, in_e, w, lo, r, o_last_b, brel_b, is_taken, tb.tbl, tb.sid);
       __syncwarp();
       for (int sl = lane; sl < tsz; sl += 32) {
-        const uint8_t id = sm.sid[sl];
+        const uint8_t id = tb.sid[sl];
         if (id != TW_SLOT_INVALID) {
           ParamView pv;
           pv.mode = prm.mode;
           pv.gauss = gauss_base ? gauss_base + (int64_t)(batch0 + (id >> 6)) * v.n_terms * TW_GAUSS_REC : nullptr;
           pv.mix = mix_base;
           pv.etab = etab;
-          sm.tbl[sl] = term_logpdf(pv, id & 63, sm.tbl[sl]);
+          tb.tbl[sl] = term_logpdf(pv, id & 63, tb.tbl[sl]);
         }
       }
       __syncwarp();
@@ -410,10 +419,10 @@ __device__ __noinline__ void stitch_search_lanes(StitchWarpSmem& sm, const tw_pa
       part.clear();
       int leaves = 0;
       bool tie = false;
-      enumerate_combos(v, w, lo_b, r_b, o_last_b, sm.sid, lane, 32, P_b,
+      enumerate_combos(v, w, lo_b, r_b, o_last_b, tb.sid, lane, 32, P_b,
                        [&](const int* c, const int64_t* ce, long long) {
                          ++leaves;
-                         const double sc = table_score(v, r_b, lo_b, sm.tbl, c, ce);
+                         const double sc = table_score(v, r_b, lo_b, tb.tbl, c, ce);
                          for (int k = 0; k < part.n; ++k) tie = tie || part.score[k] == sc;
                          tie = tie || sc != sc;
                          topk_offer_sorted(v, part, sc, c);
@@ -471,9 +480,9 @@ __device__ __noinline__ void stitch_search_lanes(StitchWarpSmem& sm, const tw_pa
     int o_last[TW_MAX_E];
     if (in_round) {
       term_table_last_offsets(v, r, o_last);
-      term_table_fill(v, in_s, in_e, w, lo, r, o_last, brel, is_taken, sm.tbl + offset, sm.sid + offset);
+      term_table_fill(v, in_s, in_e, w, lo, r, o_last, brel, is_taken, tb.tbl + offset, tb.sid + offset);
     }
-    if (lazy) {   // tables larger than the warp's slab: evaluate per leaf
+    if (lazy) {   // tables larger than the warp's StitchTables: evaluate per leaf
       ParamView pv;
       pv.mode = prm.mode;
       pv.gauss = gauss_base ? gauss_base + (int64_t)(i / TW_PARAM_BATCH) * v.n_terms * TW_GAUSS_REC : nullptr;
@@ -493,20 +502,20 @@ __device__ __noinline__ void stitch_search_lanes(StitchWarpSmem& sm, const tw_pa
     }
     __syncwarp();
     for (int s = lane; s < total; s += 32) {     // GetEpPairCost for every slot, all lanes busy
-      const uint8_t id = sm.sid[s];
+      const uint8_t id = tb.sid[s];
       if (id != TW_SLOT_INVALID) {
         ParamView pv;
         pv.mode = prm.mode;
         pv.gauss = gauss_base ? gauss_base + (int64_t)(batch0 + (id >> 6)) * v.n_terms * TW_GAUSS_REC : nullptr;
         pv.mix = mix_base;
         pv.etab = etab;
-        sm.tbl[s] = term_logpdf(pv, id & 63, sm.tbl[s]);
+        tb.tbl[s] = term_logpdf(pv, id & 63, tb.tbl[s]);
       }
     }
     __syncwarp();
     if (in_round) {
-      const double* tbl = sm.tbl + offset;
-      const uint8_t* sid = sm.sid + offset;
+      const double* tbl = tb.tbl + offset;
+      const uint8_t* sid = tb.sid + offset;
       TopK tk;
       tk.clear();
       int leaves = 0;
@@ -529,8 +538,8 @@ __device__ __noinline__ void stitch_search_lanes(StitchWarpSmem& sm, const tw_pa
 
 // Exact MWIS of a window the small-window solver does not take (more than kSmallWindow in-spans, or
 // a component with too many leaves).  Out of line like the search path: large and comparatively rare.
-__device__ __noinline__ long long stitch_mwis_large(StitchWarpSmem& sm, int E, int nw, long long node_limit, int lane) {
-  WindowBuf& wb = sm.wb;
+__device__ __noinline__ long long stitch_mwis_large(PackedWindowBuf& wb, StitchTables& tb, int E, int nw,
+                                                   long long node_limit, int lane) {
   long long nodes = 1;
   __syncwarp();
   if (lane < nw) wb.adj[lane] = window_adjacency(wb, E, nw, lane);
@@ -545,14 +554,15 @@ __device__ __noinline__ long long stitch_mwis_large(StitchWarpSmem& sm, int E, i
   for (int d = 0; d < n_def && nodes >= 0; ++d) {
     const uint32_t comp = __shfl_sync(0xffffffffu, lane == 0 ? deferred[d] : 0u, 0);
     __syncwarp();
-    nodes = mwis_component_warp(wb, E, comp, sm.tbl, node_limit, nodes, lane);
+    nodes = mwis_component_warp(wb, E, comp, tb.tbl, node_limit, nodes, lane);
   }
   return nodes;
 }
 
-__global__ void __launch_bounds__(kStitchWarps * 32, 10)
+__global__ void __launch_bounds__(kStitchWarps * 32, kStitchBlocksPerSM)
 k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_score_out spec, tw_pass_out out,
-         uint32_t* __restrict__ taken, long long node_limit, StitchUnits units, int* __restrict__ err_flag) {
+         uint32_t* __restrict__ taken, long long node_limit, StitchUnits units, StitchLayout layout,
+         StitchTables* __restrict__ tables, int* __restrict__ err_flag) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   __shared__ double etab[64];
   load_exp_table(etab);
@@ -571,7 +581,8 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
     p = u;
     if (p >= b.n_problems) return;
   }
-  StitchWarpSmem& sm = reinterpret_cast<StitchWarpSmem*>(smem_raw)[warp_in_block];
+  const StitchSlab slab{smem_raw + warp_in_block * layout.bytes};
+  StitchWarpSmem& sm = slab.fixed();
 #ifdef TW_PROFILE_PHASES
   long long _sp_t0 = clock64();
 #endif
@@ -584,7 +595,7 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
     return;
   }
   const ProbView& v = sm.v;
-  WindowBuf& wb = sm.wb;
+  PackedWindowBuf& wb = slab.window(layout);
   const int n = v.n_in, E = v.E;
   if (u1 < 0) u1 = n;
   const uint8_t* cut = cut_all + v.in_off;
@@ -597,17 +608,18 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
   // test reads three consecutive words.
   int tk_words = 0;
   for (int e = 0; e < E; ++e) tk_words += (v.n_out[e] >> 5) + 3;
-  const bool tk_smem = tk_words <= kTakenWords;
+  const bool tk_smem = tk_words <= layout.tk_words;
+  uint32_t* const tk_slab = slab.taken();
   {
     int off = 0;
     for (int e = 0; e < E; ++e) {
-      tk_base[e] = tk_smem ? sm.tk + off : taken + (v.out_off[e] >> 5) + (v.ep0 + e);
+      tk_base[e] = tk_smem ? tk_slab + off : taken + (v.out_off[e] >> 5) + (v.ep0 + e);
       off += (v.n_out[e] >> 5) + 3;
       w[e].s = v.os[e]; w[e].e = v.oe[e]; w[e].base = 0; w[e].n = v.n_out[e];
     }
   }
   if (tk_smem)
-    for (int x = lane; x < tk_words; x += 32) { sm.tk[x] = 0u; sm.tmp[x] = 0u; }
+    for (int x = lane; x < tk_words; x += 32) { tk_slab[x] = 0u; tk_slab[layout.tk_words + x] = 0u; }
   __syncwarp();
   // defaults
   for (int i = u0 + lane; i < u1; i += 32) {
@@ -683,7 +695,7 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
             const uint32_t m1 = sh ? (u0 >> (32 - sh)) | (u1 << sh) : u1;
             const uint32_t m2 = sh ? (u1 >> (32 - sh)) : 0u;
             uint32_t* tkp = tk_base[e] + q;
-            uint32_t* tmp = sm.tmp + (tkp - sm.tk);
+            uint32_t* tmp = tkp + layout.tk_words;
             if ((tkp[0] & m0) | (tkp[1] & m1) | (tkp[2] & m2)) ok = false;          // (a)
             if (m0 && (atomicOr(&tmp[0], m0) & m0)) ok = false;                     // (b)
             if (m1 && (atomicOr(&tmp[1], m1) & m1)) ok = false;
@@ -695,7 +707,7 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
         if (act && spec.used_wide[gi] == 0) {   // leave the scratch bitmap zero for the next run
           for (int e = 0; e < E; ++e) {
             const int ulo = spec.used_lo[base + e];
-            uint32_t* tmp = sm.tmp + ((tk_base[e] + (ulo >> 5)) - sm.tk);
+            uint32_t* tmp = tk_base[e] + (ulo >> 5) + layout.tk_words;
             tmp[0] = 0u; tmp[1] = 0u; tmp[2] = 0u;
           }
         }
@@ -795,7 +807,7 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
       const int32_t* ix = spec.topk_idx + TW_K * (v.tuple_off + (int64_t)i * E);
       for (int k = 0; k < cnt; ++k) {
         wb.score[lane][k] = spec.topk_score[gi * TW_K + k];
-        for (int e = 0; e < E; ++e) wb.idx[lane][k][e] = ix[k * E + e];
+        for (int e = 0; e < E; ++e) wb.at(lane, k, e) = ix[k * E + e];
       }
       if (out.topk_score) {
         out.topk_cnt[gi] = (uint8_t)cnt;
@@ -811,7 +823,7 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
     const unsigned slow_mask = __ballot_sync(0xffffffffu, active && !fast);   // (all lanes vote: the counter macro runs on lane 0 only)
     TW_SCOUNT(14, __popc(slow_mask));
     if (slow_mask)
-      stitch_search_lanes(sm, prm, out, tk_base, w, gauss_base, mix_base, etab, E, lane, ws, i, in_s, in_e,
+      stitch_search_lanes(v, wb, tables[u], prm, out, tk_base, w, gauss_base, mix_base, etab, E, lane, ws, i, in_s, in_e,
                           active && !fast, batch0);
     __syncwarp();
     TW_SPHASE(6);                                // slow path
@@ -821,9 +833,10 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
       if (lane == 0) wb.chosen[0] = (wb.cnt[0] > 0 && TW_WEIGHT_OFFSET + wb.score[0][0] > 0.0) ? 0 : -1;
     } else {
       bool solved = false;
-      if (nw <= kSmallWindow) solved = stitch_small_window(sm, E, nw, lane, &nodes);
+      if (nw <= kSmallWindow) solved = stitch_small_window(sm, wb, E, nw, lane, &nodes);
       if (!solved) {
-        nodes = stitch_mwis_large(sm, E, nw, node_limit, lane);
+        TW_SCOUNT(15, 1);
+        nodes = stitch_mwis_large(wb, tables[u], E, nw, node_limit, lane);
       }
     }
     __syncwarp();
@@ -836,7 +849,7 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
       out.mis_rank[v.in_off + i] = (int8_t)rank;
       if (rank >= 0) {
         for (int e = 0; e < E; ++e) {
-          int o = wb.idx[lane][rank][e];
+          int o = wb.at(lane, rank, e);
           out.assign[v.tuple_off + (int64_t)e * n + i] = o;
           atomicOr(&tk_base[e][o >> 5], 1u << (o & 31));
         }
@@ -953,22 +966,30 @@ extern "C" int tw_debug_stitch_phases(unsigned long long* out16, int reset) {
 }
 #endif
 
-cudaError_t setup_stitch() {
+StitchLayout stitch_layout(int e_max, int tk_words_max) {
+  StitchLayout L;
+  L.tk_words = tk_words_max < kTakenWords ? tk_words_max : kTakenWords;
+  L.wb_off = (int)sizeof(StitchWarpSmem) + 2 * L.tk_words * (int)sizeof(uint32_t);
+  L.bytes = (L.wb_off + PackedWindowBuf::packed_bytes(e_max) + 15) & ~15;
+  return L;
+}
+
+cudaError_t setup_stitch() {   // the largest slab any batch can ask for
   return cudaFuncSetAttribute(k_stitch, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              (int)(sizeof(StitchWarpSmem) * kStitchWarps));
+                              stitch_layout(TW_MAX_E, kTakenWords).bytes * kStitchWarps);
 }
 
 cudaError_t launch_stitch(const tw_batch& b, const tw_params& prm, const uint8_t* cut,
                           const tw_score_out& spec, const tw_pass_out& out, uint32_t* taken_words, size_t taken_n_words,
-                          long long node_limit, const StitchUnits& unit_buf, int max_units, int* err_flag,
-                          cudaStream_t s, int64_t& launches) {
+                          long long node_limit, const StitchUnits& unit_buf, int max_units, const StitchLayout& layout,
+                          StitchTables* tables, int* err_flag, cudaStream_t s, int64_t& launches) {
   cudaError_t e = cudaMemsetAsync(taken_words, 0, taken_n_words * sizeof(uint32_t), s);
   if (e != cudaSuccess) return e;
   if (out.counters) {
     e = cudaMemsetAsync(out.counters, 0, (size_t)b.n_problems * 4 * sizeof(int32_t), s);
     if (e != cudaSuccess) return e;
   }
-  size_t smem = sizeof(StitchWarpSmem) * kStitchWarps;
+  const size_t smem = (size_t)layout.bytes * kStitchWarps;
   StitchUnits units{nullptr, nullptr, nullptr, nullptr};
   int warps = b.n_problems;
   // Units pay when services alone cannot fill the machine (a shipped directory has 2-6 services; the
@@ -985,7 +1006,8 @@ cudaError_t launch_stitch(const tw_batch& b, const tw_params& prm, const uint8_t
     warps = max_units;
   }
   int blocks = (warps + kStitchWarps - 1) / kStitchWarps;
-  k_stitch<<<blocks, kStitchWarps * 32, smem, s>>>(b, prm, cut, spec, out, taken_words, node_limit, units, err_flag);
+  k_stitch<<<blocks, kStitchWarps * 32, smem, s>>>(b, prm, cut, spec, out, taken_words, node_limit, units, layout,
+                                                   tables, err_flag);
   return after_launch(launches);
 }
 
