@@ -78,6 +78,8 @@ __device__ __forceinline__ double sq_dist(double c, double c2, double x, double 
   return d > 0.0 ? d : 0.0;
 }
 
+// A fit's parameters.  They are the same on every lane, so each warp keeps them in a shared-memory
+// slot (the E-step reads them as broadcasts) instead of 4K registers per thread.
 struct Fit {
   double mu[KC], pc[KC], logpc[KC], logw[KC];
 };
@@ -327,31 +329,49 @@ __device__ __forceinline__ void lloyd_centres(const double* __restrict__ x, int 
   TW_GPHASE(1);
 }
 
-// parameters from the M-step sums.  S0 = sum r, S1 = sum r x' (x' = x - shift).
+// v[lane] on lanes 0..K-1, v[0] on the others: hands each of the first K lanes its component of a
+// warp-uniform per-component array
+template <int K>
+__device__ __forceinline__ double lane_component(const double* v) {
+  const int lane = threadIdx.x & 31;
+  double r = v[0];
+#pragma unroll
+  for (int c = 1; c < K; ++c) r = lane == c ? v[c] : r;
+  return r;
+}
+
+// parameters from the M-step sums, component c on lane c (lanes >= K idle), written to the warp's
+// shared slot f; the arguments are lane c's component.  nk = sum r, mup = sum r x' / nk
+// (x' = x - shift), tot = nk summed over the components in order c = 0..K-1.
 //   'diag': S2 = sum r x^2 with shift = 0 and cov = S2/nk - mu^2 + reg — scikit-learn's own
 //           avg_X2 - means^2 formula (_estimate_gaussian_covariances_diag);
 //   'full': S2 = sum r (x' - mu')^2 from a second sweep (_estimate_gaussian_covariances_full),
 //           so a component of identical samples gets cov = reg_covar exactly, as in the library.
-template <bool FULL>
-__device__ __forceinline__ bool params_from_stats(Fit& f, int k, int n, const double* nk, const double* mup,
-                                                  const double* S2, double shift, bool init) {
-  double tot = 0.0;
+// The roundings are spelled out so that the fits keep the bits they had when every lane evaluated
+// every component with the plain expressions: there -O3 contracted component 0's S2/nk - mup^2 into
+// one fused multiply-add and left the other components' product and difference separately rounded.
+// The 'diag' BIC arg-min is ill-conditioned on terms with few distinct delays, so one ulp of one
+// covariance can move the selected K (tests/gmm_conditioning.py).
+template <int K, bool FULL>
+__device__ __forceinline__ bool params_from_stats(Fit& f, int n, double nk, double mup, double S2, double tot,
+                                                  double shift, bool init) {
+  const int c = threadIdx.x & 31;
   bool ok = true;
-#pragma unroll
-  for (int c = 0; c < KC; ++c)
-    if (c < k) tot += nk[c];
-#pragma unroll
-  for (int c = 0; c < KC; ++c) {
-    if (c < k) {
-      double cov = FULL ? S2[c] / nk[c] + kRegCovar : S2[c] / nk[c] - mup[c] * mup[c] + kRegCovar;
-      if (!(cov > 0.0)) ok = false;
-      f.mu[c] = mup[c] + shift;
-      f.pc[c] = 1.0 / sqrt(cov);
-      f.logpc[c] = log(f.pc[c]);
-      f.logw[c] = log(init ? nk[c] / (double)n : nk[c] / tot);
-    }
+  __syncwarp();                      // the E-step reads of the previous parameters are done
+  if (c < K) {
+    const double q = __ddiv_rn(S2, nk);
+    const double cov = FULL     ? __dadd_rn(q, kRegCovar)
+                       : c == 0 ? __dadd_rn(fma(-mup, mup, q), kRegCovar)
+                                : __dadd_rn(__dsub_rn(q, __dmul_rn(mup, mup)), kRegCovar);
+    ok = cov > 0.0;
+    const double pc = __ddiv_rn(1.0, sqrt(cov));
+    f.mu[c] = __dadd_rn(mup, shift);
+    f.pc[c] = pc;
+    f.logpc[c] = log(pc);
+    f.logw[c] = log(__ddiv_rn(nk, init ? (double)n : tot));
   }
-  return ok;
+  __syncwarp();
+  return __all_sync(kFull, ok);
 }
 
 // E-step of one sample.  a[c] <- exp(w_c - max w) with w_c the weighted log-probabilities (sklearn
@@ -417,6 +437,7 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
   if (n < 2 || n < k) return false;
   const double shift = FULL ? mean : 0.0;
   double S0[KC], S1[KC], S2[KC], nk[KC], mup[KC];
+  double my_nk, my_mup, my_s2;       // this lane's component (lanes 0..K-1)
   TW_GPHASE_BEGIN;
   {
     TW_GCOUNT(7, 1);
@@ -438,12 +459,16 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
       }
     });
 #pragma unroll
-    for (int c = 0; c < KC; ++c) {
+    for (int c = 0; c < K; ++c) {
       nk[c] = wsum(S0[c]) + 10.0 * kDblEps;
-      mup[c] = wsum(S1[c]) / nk[c];
+      S1[c] = wsum(S1[c]);
       S2[c] = wsum(S2[c]);
     }
+    my_nk = lane_component<K>(nk);
+    my_mup = __ddiv_rn(lane_component<K>(S1), my_nk);
     if (FULL) {   // second sweep: sum of squared deviations from the new means
+#pragma unroll
+      for (int c = 0; c < K; ++c) mup[c] = __shfl_sync(kFull, my_mup, c);
 #pragma unroll
       for (int c = 0; c < KC; ++c) S2[c] = 0.0;
       sweep2(x, n, [&](double x0, double x1, bool v1, int) {
@@ -460,10 +485,11 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
         }
       });
 #pragma unroll
-      for (int c = 0; c < KC; ++c) S2[c] = wsum(S2[c]);
+      for (int c = 0; c < K; ++c) S2[c] = wsum(S2[c]);
     }
+    my_s2 = lane_component<K>(S2);
   }
-  if (!params_from_stats<FULL>(f, k, n, nk, mup, S2, shift, true)) return false;
+  if (!params_from_stats<K, FULL>(f, n, my_nk, my_mup, my_s2, 0.0, shift, true)) return false;
   TW_GPHASE(2);
   double lower = -INFINITY;
   int em_sweeps = 0;
@@ -496,23 +522,26 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
       }
     }
     lower = wsum(ls.total()) / (double)n;
+    double tot = 0.0;
 #pragma unroll
-    for (int c = 0; c < KC; ++c) {
-      if (c < K) {
-        nk[c] = wsum(S0[c]) + 10.0 * kDblEps;
-        const double s1 = wsum(S1[c]);
-        S2[c] = wsum(S2[c]);
-        if (FULL) {
-          const double delta = s1 / nk[c];
-          S2[c] -= delta * s1;
-          if (S2[c] < 0.0) S2[c] = 0.0;
-          mup[c] = (f.mu[c] + delta) - shift;
-        } else {
-          mup[c] = s1 / nk[c];
-        }
-      }
+    for (int c = 0; c < K; ++c) {
+      nk[c] = wsum(S0[c]) + 10.0 * kDblEps;
+      tot += nk[c];
+      S1[c] = wsum(S1[c]);
+      S2[c] = wsum(S2[c]);
     }
-    if (!params_from_stats<FULL>(f, k, n, nk, mup, S2, shift, false)) {
+    my_nk = lane_component<K>(nk);
+    const double s1 = lane_component<K>(S1);
+    my_s2 = lane_component<K>(S2);
+    if (FULL) {      // S2 - delta s1 is one fused multiply-add, as -O3 contracted it before
+      const double delta = __ddiv_rn(s1, my_nk);
+      my_s2 = fma(-delta, s1, my_s2);
+      if (my_s2 < 0.0) my_s2 = 0.0;
+      my_mup = __dsub_rn(__dadd_rn(f.mu[lane < K ? lane : 0], delta), shift);
+    } else {
+      my_mup = __ddiv_rn(s1, my_nk);
+    }
+    if (!params_from_stats<K, FULL>(f, n, my_nk, my_mup, my_s2, tot, shift, false)) {
       if (lane == 0) atomicAdd(&g_gmm_em_evals, (unsigned long long)it * (unsigned long long)n * K);
       return false;
     }
@@ -631,9 +660,9 @@ __global__ void k_gmm_draws(int n_problems, const int32_t* __restrict__ prob_ep_
 // few hundred instructions.  The fused single-kernel fit of the first versions (10 k SASS
 // instructions for K = 5, warps spread over three different hot loops) lost issue slots to
 // instruction fetch (stall_no_inst).
-#ifndef TW_GMM_MINB
-#define TW_GMM_MINB 1
-#endif
+// Blocks of 128 threads per SM that the EM kernels are compiled for: 4 (16 warps) for K = 4, 5, whose
+// register footprint would otherwise allow only 3; the smaller K reach 16 warps unconstrained.
+constexpr int em_min_blocks(int K) { return K >= 4 ? 4 : 1; }
 
 // Which fit a warp works on.  Model selection (list == nullptr): warp w -> term w, active iff the
 // reference tries K components for it (K <= min(#unique, 5)), draws at the term's stream position.
@@ -717,11 +746,12 @@ k_gmm_lloyd(FitSel sel, const int64_t* __restrict__ term_sample_off, const doubl
 
 // 'diag' fit + BIC of the terms that try K components
 template <int K>
-__global__ void __launch_bounds__(128, TW_GMM_MINB)
+__global__ void __launch_bounds__(128, em_min_blocks(K))
 k_gmm_bic(FitSel sel, const int64_t* __restrict__ term_sample_off, const double* __restrict__ delays,
           const int32_t* __restrict__ counts, const double* __restrict__ mean_var,
           const double* __restrict__ cen_in, double* __restrict__ bic_out) {
   __shared__ double tab[64];
+  __shared__ Fit fits[128 / 32];
   load_exp_table(tab);
   const int w = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) >> 5);
   if (w >= sel.n_terms) return;
@@ -733,7 +763,7 @@ k_gmm_bic(FitSel sel, const int64_t* __restrict__ term_sample_off, const double*
     double cen[KC];
 #pragma unroll
     for (int j = 0; j < KC; ++j) cen[j] = j < K ? cen_in[(size_t)t * KC + j] : 0.0;
-    Fit f;
+    Fit& f = fits[threadIdx.x >> 5];
     double sc = 0.0;
     if (em_fit<K, false>(delays + term_sample_off[t], n, mean_var[2 * t], cen, tab, f, true, &sc))
       bic = -2.0 * sc * (double)n + (double)(3 * K - 1) * log((double)n);   // GaussianMixture.bic, 'diag'
@@ -780,11 +810,12 @@ __global__ void k_gmm_group(int n_terms, const int32_t* __restrict__ best_k, con
 
 // final 'full' fit of the terms whose BIC arg-min is K: dense warps over the grouped list
 template <int K>
-__global__ void __launch_bounds__(128, TW_GMM_MINB)
+__global__ void __launch_bounds__(128, em_min_blocks(K))
 k_gmm_final(FitSel sel, const int64_t* __restrict__ term_sample_off, const double* __restrict__ delays,
             const int32_t* __restrict__ counts, const double* __restrict__ mean_var,
             const double* __restrict__ cen_in, double* __restrict__ mix_out, int32_t* __restrict__ n_selected_out) {
   __shared__ double tab[64];
+  __shared__ Fit fits[128 / 32];
   load_exp_table(tab);
   const unsigned w = (blockIdx.x * (unsigned)blockDim.x + threadIdx.x) >> 5;
   if (w >= sel.hist[K]) return;
@@ -797,7 +828,7 @@ k_gmm_final(FitSel sel, const int64_t* __restrict__ term_sample_off, const doubl
   double cen[KC];
 #pragma unroll
   for (int j = 0; j < KC; ++j) cen[j] = j < K ? cen_in[(size_t)t * KC + j] : 0.0;
-  Fit f;
+  Fit& f = fits[threadIdx.x >> 5];
   const bool ok = em_fit<K, true>(delays + term_sample_off[t], n, mean_var[2 * t], cen, tab, f, false, nullptr);
   if (lane == 0) {
     double* rec = mix_out + (size_t)t * TW_MIX_REC;
