@@ -79,7 +79,7 @@ class OracleBatch:
         nt = int(hb.prob_tuple_off[-1])
         res = dict(topk_score=np.full((n, _abi.TW_K), np.nan), topk_idx=np.full(_abi.TW_K * nt, -1, np.int32),
                    topk_cnt=np.zeros(n, np.uint8), n_feasible=np.zeros(n, np.int32), cut=np.zeros(n, np.uint8))
-        out = _abi.TwScoreOut(*[_ptr(res[k]) for k in ("topk_score", "topk_idx", "topk_cnt", "n_feasible", "cut")])
+        out = _abi.fill(_abi.TwScoreOut, res)
         have = gauss is not None or mix is not None
         prm = self._params_struct(gauss, mix) if have else None
         for p in range(hb.n_problems):
@@ -98,8 +98,7 @@ class OracleBatch:
                    topk_idx=np.full(_abi.TW_K * nt, -1, np.int32) if want_topk else None,
                    topk_cnt=np.zeros(n, np.uint8) if want_topk else None,
                    counters=np.zeros((hb.n_problems, 4), np.int32))
-        out = _abi.TwPassOut(*[_ptr(res[k]) for k in ("assign", "mis_rank", "n_cand", "topk_score", "topk_idx",
-                                                      "topk_cnt", "counters")])
+        out = _abi.fill(_abi.TwPassOut, res)
         prm = self._params_struct(gauss, mix)
         cut = np.ascontiguousarray(cut, np.uint8)
         for p in range(hb.n_problems):
@@ -155,13 +154,11 @@ def find_assignments(hb: HostBatch, seed_select=10, threads=1, want_topk=True):
     res = dict(assign=np.full(nt, -1, np.int32), mis_rank=np.full(n, -1, np.int8), n_cand=np.zeros(n, np.int32),
                counters=np.zeros((hb.n_problems, 4), np.int32), n_cand_total=np.zeros(n, np.int32),
                mix=np.zeros((nterm, _abi.TW_MIX_REC)))
+    final = _abi.fill(_abi.TwPassOut, res)            # the final pass writes no top-K lists
     if want_topk:
         res.update(topk_score=np.full((n, _abi.TW_K), np.nan), topk_idx=np.full(_abi.TW_K * nt, -1, np.int32),
                    topk_cnt=np.zeros(n, np.uint8))
-    final = _abi.TwPassOut(_ptr(res["assign"]), _ptr(res["mis_rank"]), _ptr(res["n_cand"]), None, None, None,
-                           _ptr(res["counters"]))
-    top = _abi.TwScoreOut(_ptr(res.get("topk_score")), _ptr(res.get("topk_idx")), _ptr(res.get("topk_cnt")),
-                          None, None)
+    top = _abi.fill(_abi.TwScoreOut, res)
     st = batch_struct(hb, lambda name: _ptr(hb.arrays[name]))
     _check(L.two_find_assignments(C.byref(st), C.c_uint32(seed_select), C.c_int(threads), C.byref(final),
                                   C.byref(top) if want_topk else None, _ptr(res["n_cand_total"]), _ptr(res["mix"])),

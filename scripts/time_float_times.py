@@ -84,9 +84,8 @@ def main():
 
     # the conversion kernels alone: re-bind the resident batch under the profiler
     eng = Engine(0)
-    d = {k: torch.from_numpy(np.ascontiguousarray(v.view(np.int32) if v.dtype == np.uint32 else v)).to(eng.device)
-         for k, v in hb.arrays.items()}
-    eng.bind(hb, device_arrays=d)
+    eng.bind(hb)
+    d = eng.d
     torch.cuda.synchronize()
     binds = 5
     with profile(activities=[ProfilerActivity.CUDA]) as prof:

@@ -43,7 +43,7 @@ class EmulBatch(OracleBatch):
         nt = int(hb.prob_tuple_off[-1])
         res = dict(topk_score=np.full((n, _abi.TW_K), np.nan), topk_idx=np.full(_abi.TW_K * nt, -1, np.int32),
                    topk_cnt=np.zeros(n, np.uint8), n_feasible=np.zeros(n, np.int32), cut=np.zeros(n, np.uint8))
-        out = _abi.TwScoreOut(*[_ptr(res[k]) for k in ("topk_score", "topk_idx", "topk_cnt", "n_feasible", "cut")])
+        out = _abi.fill(_abi.TwScoreOut, res)
         have = gauss is not None or mix is not None
         prm = self._params_struct(gauss, mix) if have else None
         self.overflow = []
@@ -70,8 +70,7 @@ class EmulBatch(OracleBatch):
                    topk_idx=np.full(_abi.TW_K * nt, -1, np.int32) if want_topk else None,
                    topk_cnt=np.zeros(n, np.uint8) if want_topk else None,
                    counters=np.zeros((hb.n_problems, 4), np.int32))
-        out = _abi.TwPassOut(*[_ptr(res[k]) for k in ("assign", "mis_rank", "n_cand", "topk_score", "topk_idx",
-                                                      "topk_cnt", "counters")])
+        out = _abi.fill(_abi.TwPassOut, res)
         prm = self._params_struct(gauss, mix)
         cut = np.ascontiguousarray(cut, np.uint8)
         for p in range(hb.n_problems):
@@ -96,10 +95,8 @@ def skip_solve(in_start, in_end, out_start, out_end, preds, wins, counts, pair, 
                topk_cnt=np.zeros(n, np.uint8), counters=np.zeros((1, 4), np.int32),
                top2_score=np.full((n, _abi.TW_K), np.nan), top2_idx=np.full(_abi.TW_K * nt, -1, np.int32),
                top2_cnt=np.zeros(n, np.uint8), cut=np.zeros(n, np.uint8))
-    sd = _abi.TwSkipDesc(*[_ptr(host[f]) for f, _ in _abi.TwSkipDesc._fields_])
-    so = _abi.TwSkipOut(_abi.TwPassOut(*[_ptr(out[k]) for k in ("assign", "mis_rank", "n_cand", "topk_score", "topk_idx",
-                                                                 "topk_cnt", "counters")]),
-                        _ptr(out["top2_score"]), _ptr(out["top2_idx"]), _ptr(out["top2_cnt"]), _ptr(out["cut"]))
+    sd = _abi.fill(_abi.TwSkipDesc, host)
+    so = _abi.fill(_abi.TwSkipOut, out)
     st = batch_struct(hb, lambda name: _ptr(hb.arrays[name]))
     L = lib()
     L.twe_skip_solve.restype = C.c_int

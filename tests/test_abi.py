@@ -80,15 +80,19 @@ def test_terms_follow_reference_order():
     assert not p.is_primary(0, 2) and p.is_primary(1, 2)
 
 
-def test_batch_slice_equals_rebuilt_batch():
-    """HostBatch.slice(lo, hi) == build_batch(problems[lo:hi]) array for array (chunked solver, api.py)."""
+def _mixed_blocks():
     from traceweaver_b200 import synth
-    from traceweaver_b200.batch import build_batch, build_batch_from_blocks
     blocks = [synth.make_block("hotel_frontend", 3, 40, 100.0, seed=1),
               synth.make_block("media_nginx", 4, 25, 100.0, seed=2),
               synth.make_block("single", 2, 30, 100.0, seed=3)]
+    return blocks, [blk.problem(s) for blk in blocks for s in range(blk.in_start.shape[0])]
+
+
+def test_batch_slice_equals_rebuilt_batch():
+    """HostBatch.slice(lo, hi) == build_batch(problems[lo:hi]) array for array (chunked solver, api.py)."""
+    from traceweaver_b200.batch import build_batch, build_batch_from_blocks
+    blocks, probs = _mixed_blocks()
     hb = build_batch_from_blocks(blocks)
-    probs = [blk.problem(s) for blk in blocks for s in range(blk.in_start.shape[0])]
     full = build_batch(probs)
     for k, v in full.arrays.items():
         assert np.array_equal(hb.arrays[k], v), k
@@ -100,3 +104,25 @@ def test_batch_slice_equals_rebuilt_batch():
             for k, v in want.arrays.items():
                 assert got.arrays[k].dtype == v.dtype, k
                 assert np.array_equal(got.arrays[k], v), k
+
+
+def test_trace_lists_share_the_batch_offsets():
+    """truth.TraceLists derives the offset tables build_batch derives; as a batch without term tables
+    its TwBatch has NULL term pointers and n_term_total = 0."""
+    from traceweaver_b200.truth import TraceLists
+    _, probs = _mixed_blocks()
+    tl = TraceLists([dict(in_start=p.in_start, in_end=p.in_end, out_start=p.out_start, out_end=p.out_end)
+                     for p in probs],
+                    [np.arange(p.n_in, dtype=np.int32) for p in probs],
+                    [[np.arange(len(o), dtype=np.int32) for o in p.out_start] for p in probs],
+                    max(p.n_in for p in probs))
+    full = build_batch(probs)
+    for k in ("prob_in_off", "prob_ep_off", "prob_tuple_off", "ep_out_off"):
+        assert tl.arrays[k].dtype == full.arrays[k].dtype, k
+        assert np.array_equal(tl.arrays[k], full.arrays[k]), k
+    st = batch_struct(tl, lambda n: tl.arrays[n].ctypes.data)
+    assert st.ep_term_off is None and st.ep_pred_mask is None and st.term_src is None
+    assert st.n_term_total == 0
+    assert st.in_start == tl.arrays["in_start"].ctypes.data
+    assert (st.n_problems, st.n_ep_total, st.n_in_total, st.n_out_total) == (
+        len(probs), int(full.prob_ep_off[-1]), int(full.prob_in_off[-1]), int(full.ep_out_off[-1]))

@@ -76,6 +76,21 @@ class TwTraceKeys(C.Structure):
                 ("n_traces", C.c_int32), ("reserved0", C.c_int32)]
 
 
+def fill(cls, arrays, **values):
+    """A `cls` instance built by field name: each pointer field points at `arrays[name]` (a numpy
+    array on the host or a torch tensor on the device; NULL when the name is missing or None), a
+    nested structure is filled from the same mapping, and the other fields come from `values`."""
+    s = cls(**values)
+    for name, typ in cls._fields_:
+        if typ is P:
+            a = arrays.get(name)
+            if a is not None:
+                setattr(s, name, a.data_ptr() if hasattr(a, "data_ptr") else a.ctypes.data)
+        elif issubclass(typ, C.Structure):
+            setattr(s, name, fill(typ, arrays))
+    return s
+
+
 class TwError(RuntimeError):
     def __init__(self, code, where, detail=""):
         self.code = code

@@ -24,11 +24,8 @@ import torch
 
 from . import _abi
 from .batch import HostBatch
-from .engine import Engine
+from .engine import Engine, _to_device
 from .predictor import solve_bound
-
-SPAN_ARRAYS = ("in_start", "in_end", "out_start", "out_end")
-RESULTS = ("assign", "topk_idx", "topk_cnt", "n_cand", "counters", "mis_rank")
 
 
 class BatchSolver:
@@ -142,12 +139,8 @@ class BatchSolver:
                     d[name] = p.to(dev, non_blocking=True)        # H2D inside the caller's timed region
                     h2d += p.numel() * p.element_size()
                 eng.bind(sub, device_arrays=d)
-                ta = to = None
-                if single:
-                    ta = None if truth_assign is None else torch.from_numpy(
-                        np.ascontiguousarray(truth_assign, np.int32)).to(dev)
-                    to = None if term_order is None else torch.from_numpy(
-                        np.ascontiguousarray(term_order, np.int32)).to(dev)
+                inputs = _to_device({k: None if v is None else np.asarray(v, np.int32)
+                                     for k, v in (("truth_assign", truth_assign), ("term_order", term_order))}, dev)
                 i0, t0 = int(hb.prob_in_off[lo]), int(hb.prob_tuple_off[lo])
                 i1, t1 = int(hb.prob_in_off[hi]), int(hb.prob_tuple_off[hi])
 
@@ -166,8 +159,7 @@ class BatchSolver:
                             t.record_stream(self._copy_stream)
                             out[name][b0:b1].copy_(t, non_blocking=True)
 
-                res = solve_bound(eng, seed_select=self.seed_select, truth_assign=ta, term_order=to, check=False,
-                                  after_score=copy_topk)
+                res = solve_bound(eng, seed_select=self.seed_select, check=False, after_score=copy_topk, **inputs)
                 d2h += sum(res[k].numel() * res[k].element_size()
                            for k in ("topk_idx", "topk_cnt") + (("topk_score",) if want_scores else ()))
                 for name, (b0, b1) in (("assign", (t0, t1)), ("n_cand", (i0, i1)), ("counters", (lo, hi)),

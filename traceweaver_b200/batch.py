@@ -154,66 +154,68 @@ class HostBatch:
         return HostBatch(problems=probs, arrays=arrays)
 
 
+def _cumulative(counts, dtype):
+    return np.concatenate([[0], np.cumsum(counts)]).astype(dtype)
+
+
+def offset_tables(n_in, E, n_out, n_term=None):
+    """The offset tables of tw_batch from the counts: n_in and E per problem, n_out per ep (problem by
+    problem, topological order).  With n_term (terms per ep) also the term tables: ep_term_off,
+    prob_gauss_off (one record per term and 100-span batch) and term_sample_off (a term holds up to
+    n_in samples of its problem, tw_delays)."""
+    n_in = np.asarray(n_in, np.int64)
+    E = np.asarray(E, np.int64)
+    t = dict(prob_in_off=_cumulative(n_in, np.int64), prob_ep_off=_cumulative(E, np.int32),
+             prob_tuple_off=_cumulative(n_in * E, np.int64), ep_out_off=_cumulative(n_out, np.int64))
+    if n_term is not None:
+        t["ep_term_off"] = _cumulative(n_term, np.int32)
+        prob_terms = np.diff(t["ep_term_off"].astype(np.int64)[t["prob_ep_off"]])
+        n_batches = (n_in + _abi.TW_PARAM_BATCH - 1) // _abi.TW_PARAM_BATCH
+        t["prob_gauss_off"] = _cumulative(n_batches * prob_terms, np.int64)
+        t["term_sample_off"] = _cumulative(np.repeat(n_in, prob_terms), np.int64)
+    return t
+
+
 def build_batch(problems: Sequence[Problem], validate=True) -> HostBatch:
-    P = len(problems)
-    if P == 0:
+    if len(problems) == 0:
         raise ValueError("empty batch")
     if validate:
         for p in problems:
             p.validate()
-    prob_in_off = np.zeros(P + 1, np.int64)
-    prob_ep_off = np.zeros(P + 1, np.int32)
-    prob_tuple_off = np.zeros(P + 1, np.int64)
-    ep_out_off = [0]
-    ep_term_off = [0]
-    ep_pred_mask = []
-    term_src = []
-    for i, p in enumerate(problems):
-        prob_in_off[i + 1] = prob_in_off[i] + p.n_in
-        prob_ep_off[i + 1] = prob_ep_off[i] + p.E
-        prob_tuple_off[i + 1] = prob_tuple_off[i] + p.n_in * p.E
+    n_out, n_term, ep_pred_mask, term_src = [], [], [], []
+    for p in problems:
         terms = p.terms()
         for e in range(p.E):
-            ep_out_off.append(ep_out_off[-1] + int(p.out_start[e].shape[0]))
+            n_out.append(int(p.out_start[e].shape[0]))
             mask = 0
             for b in p.preds[e]:
                 mask |= 1 << b
             ep_pred_mask.append(mask)
             mine = [src for (ee, src) in terms if ee == e]
             term_src.extend(mine)
-            ep_term_off.append(ep_term_off[-1] + len(mine))
+            n_term.append(len(mine))
     tdt = _time_dtype([a for p in problems for a in [p.in_start, p.in_end] + list(p.out_start) + list(p.out_end)])
-    arrays = dict(
-        prob_in_off=prob_in_off, prob_ep_off=prob_ep_off, prob_tuple_off=prob_tuple_off,
-        ep_out_off=np.asarray(ep_out_off, np.int64), ep_term_off=np.asarray(ep_term_off, np.int32),
+    arrays = offset_tables([p.n_in for p in problems], [p.E for p in problems], n_out, n_term)
+    arrays.update(
         ep_pred_mask=np.asarray(ep_pred_mask, np.uint32), term_src=np.asarray(term_src, np.int8),
         in_start=np.ascontiguousarray(np.concatenate([p.in_start for p in problems]), tdt),
         in_end=np.ascontiguousarray(np.concatenate([p.in_end for p in problems]), tdt),
         out_start=np.ascontiguousarray(np.concatenate([s for p in problems for s in p.out_start]), tdt),
         out_end=np.ascontiguousarray(np.concatenate([s for p in problems for s in p.out_end]), tdt),
     )
-    n_batches = (np.diff(prob_in_off) + _abi.TW_PARAM_BATCH - 1) // _abi.TW_PARAM_BATCH
-    n_terms = np.diff(np.asarray(ep_term_off, np.int64)[prob_ep_off])
-    arrays["prob_gauss_off"] = np.concatenate([[0], np.cumsum(n_batches * n_terms)]).astype(np.int64)
-    # sample capacity of a term = n_in of its problem (tw_delays)
-    term_prob = np.repeat(np.arange(P), n_terms)
-    arrays["term_sample_off"] = np.concatenate(
-        [[0], np.cumsum(np.diff(prob_in_off)[term_prob])]).astype(np.int64)
     return HostBatch(problems=list(problems), arrays=arrays)
 
 
 def batch_struct(hb: HostBatch, ptr):
-    """Fill a TwBatch with pointers produced by `ptr(name)` (host or device)."""
+    """Fill a TwBatch with pointers produced by `ptr(name)` (host or device).  A batch without term
+    tables (truth.TraceLists) gets NULL ep_term_off / ep_pred_mask / term_src and n_term_total = 0."""
     a = hb.arrays
-    s = _abi.TwBatch()
-    s.n_problems = hb.n_problems
-    s.n_ep_total = int(a["prob_ep_off"][-1])
-    s.n_term_total = int(a["ep_term_off"][-1])
-    s.n_in_total = int(a["prob_in_off"][-1])
-    s.n_out_total = int(a["ep_out_off"][-1])
-    for name in ("prob_in_off", "prob_ep_off", "prob_tuple_off", "ep_out_off", "ep_term_off",
-                 "ep_pred_mask", "term_src", "in_start", "in_end", "out_start", "out_end"):
-        setattr(s, name, ptr(name))
+    s = _abi.TwBatch(n_problems=hb.n_problems, n_ep_total=int(a["prob_ep_off"][-1]),
+                     n_term_total=int(a["ep_term_off"][-1]) if "ep_term_off" in a else 0,
+                     n_in_total=int(a["prob_in_off"][-1]), n_out_total=int(a["ep_out_off"][-1]))
+    for name, typ in _abi.TwBatch._fields_:
+        if typ is _abi.P and name in a:
+            setattr(s, name, ptr(name))
     return s
 
 
@@ -237,8 +239,7 @@ class ServiceBlock:
 
 def build_batch_from_blocks(blocks: Sequence[ServiceBlock]) -> HostBatch:
     """Same arrays as build_batch([...problems of every block...]) without per-problem Python work."""
-    prob_in, prob_ep, prob_tuple = [0], [0], [0]
-    ep_out, ep_term, ep_pred, term_src = [0], [0], [], []
+    n_in, n_ep, n_out, n_term, ep_pred, term_src = [], [], [], [], [], []
     ins, ine, outs, oute = [], [], [], []
     for blk in blocks:
         S, n = blk.in_start.shape
@@ -249,15 +250,10 @@ def build_batch_from_blocks(blocks: Sequence[ServiceBlock]) -> HostBatch:
         terms = tmpl.terms()
         per_ep_terms = [[src for (ee, src) in terms if ee == e] for e in range(E)]
         masks = [sum(1 << b for b in blk.preds[e]) for e in range(E)]
-        base_in, base_ep, base_tuple = prob_in[-1], prob_ep[-1], prob_tuple[-1]
-        prob_in.extend(base_in + n * np.arange(1, S + 1))
-        prob_ep.extend(base_ep + E * np.arange(1, S + 1))
-        prob_tuple.extend(base_tuple + n * E * np.arange(1, S + 1))
-        base_out, base_term = ep_out[-1], ep_term[-1]
-        ep_out.extend(base_out + n * np.arange(1, S * E + 1))
-        cum = np.cumsum([len(t) for t in per_ep_terms])
-        nt = int(cum[-1])
-        ep_term.extend((base_term + nt * np.arange(S)[:, None] + cum[None, :]).reshape(-1))
+        n_in.append(np.full(S, n))
+        n_ep.append(np.full(S, E))
+        n_out.append(np.full(S * E, n))
+        n_term.append(np.tile([len(t) for t in per_ep_terms], S))
         ep_pred.extend(masks * S)
         term_src.extend([src for t in per_ep_terms for src in t] * S)
         ins.append(blk.in_start.reshape(-1))
@@ -266,24 +262,14 @@ def build_batch_from_blocks(blocks: Sequence[ServiceBlock]) -> HostBatch:
         outs.append(np.stack(blk.out_start, axis=1).reshape(-1))
         oute.append(np.stack(blk.out_end, axis=1).reshape(-1))
     tdt = _time_dtype(ins + ine + outs + oute)
-    arrays = dict(
-        prob_in_off=np.asarray(prob_in, np.int64), prob_ep_off=np.asarray(prob_ep, np.int32),
-        prob_tuple_off=np.asarray(prob_tuple, np.int64), ep_out_off=np.asarray(ep_out, np.int64),
-        ep_term_off=np.asarray(ep_term, np.int32), ep_pred_mask=np.asarray(ep_pred, np.uint32),
-        term_src=np.asarray(term_src, np.int8),
+    arrays = offset_tables(np.concatenate(n_in), np.concatenate(n_ep), np.concatenate(n_out), np.concatenate(n_term))
+    arrays.update(
+        ep_pred_mask=np.asarray(ep_pred, np.uint32), term_src=np.asarray(term_src, np.int8),
         in_start=np.ascontiguousarray(np.concatenate(ins), tdt),
         in_end=np.ascontiguousarray(np.concatenate(ine), tdt),
         out_start=np.ascontiguousarray(np.concatenate(outs), tdt),
         out_end=np.ascontiguousarray(np.concatenate(oute), tdt))
-    P = len(prob_in) - 1
-    n_in = np.diff(arrays["prob_in_off"])
-    n_batches = (n_in + _abi.TW_PARAM_BATCH - 1) // _abi.TW_PARAM_BATCH
-    n_terms = np.diff(arrays["ep_term_off"].astype(np.int64)[arrays["prob_ep_off"]])
-    arrays["prob_gauss_off"] = np.concatenate([[0], np.cumsum(n_batches * n_terms)]).astype(np.int64)
-    term_prob = np.repeat(np.arange(P), n_terms)
-    arrays["term_sample_off"] = np.concatenate([[0], np.cumsum(n_in[term_prob])]).astype(np.int64)
-    hb = HostBatch(problems=_ProblemCount(P), arrays=arrays)
-    return hb
+    return HostBatch(problems=_ProblemCount(len(arrays["prob_in_off"]) - 1), arrays=arrays)
 
 
 class _ProblemCount:

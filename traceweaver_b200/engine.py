@@ -9,13 +9,25 @@ from . import _abi, _lib
 from .batch import SPAN_ARRAYS, HostBatch, batch_struct
 
 
-def _to_device(a: np.ndarray, device, pinned=False):
-    if a.dtype == np.uint32:
-        a = a.view(np.int32)
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    if pinned:
-        t = t.pin_memory()
-    return t.to(device, non_blocking=pinned)
+def _to_device(arrays, device, resident=None, pinned=()):
+    """Device tensors of a name -> host array mapping; the one way host arrays reach the device.
+    None entries are left out, a name in `resident` adopts the tensor given there (already on the
+    device), names in `pinned` go through page-locked staging (asynchronous copy).  uint32 arrays
+    travel as int32: torch has no uint32 tensors, the kernels read the bits."""
+    d = {}
+    for name, a in arrays.items():
+        if a is None:
+            continue
+        if resident and name in resident:
+            d[name] = resident[name]
+            continue
+        if a.dtype == np.uint32:
+            a = a.view(np.int32)
+        t = torch.from_numpy(np.ascontiguousarray(a))
+        if name in pinned:
+            t = t.pin_memory()
+        d[name] = t.to(device, non_blocking=name in pinned)
+    return d
 
 
 def _p(t):
@@ -75,17 +87,11 @@ class Engine:
         already resident on the device for the four span arrays.  A batch with float64 span arrays
         (fractional microseconds) is bound through tw_engine_bind_f64."""
         self.hb = hb
-        d = {}
-        for name, a in hb.arrays.items():
-            if device_arrays and name in device_arrays:
-                d[name] = device_arrays[name]
-            else:
-                d[name] = _to_device(a, self.device, pinned=pinned and name in SPAN_ARRAYS)
-        self.d = d
+        self.d = d = _to_device(hb.arrays, self.device, device_arrays, SPAN_ARRAYS if pinned else ())
         self.dev_struct = batch_struct(hb, lambda n: d[n].data_ptr())
         self.host_struct = batch_struct(hb, lambda n: hb.arrays[n].ctypes.data)
         if hb.float_times:
-            self.times_struct = _abi.TwTimesF64(*[d[n].data_ptr() for n in SPAN_ARRAYS])
+            self.times_struct = _abi.fill(_abi.TwTimesF64, d)
             _lib.check(self.lib.tw_engine_bind_f64(self.h, C.byref(self.dev_struct), C.byref(self.host_struct),
                                                    C.byref(self.times_struct), self.stream), "tw_engine_bind_f64")
         else:
@@ -127,10 +133,10 @@ class Engine:
 
     def params_from_host(self, gauss=None, mix=None) -> Params:
         if mix is not None:
-            t = _to_device(np.asarray(mix, np.float64).reshape(-1, _abi.TW_MIX_REC), self.device)
-            return Params(_abi.TW_PARAMS_MIXTURE, t, self.d["prob_gauss_off"])
-        t = _to_device(np.asarray(gauss, np.float64).reshape(-1, _abi.TW_GAUSS_REC), self.device)
-        return Params(_abi.TW_PARAMS_GAUSS_BATCHED, t, self.d["prob_gauss_off"])
+            t = _to_device(dict(mix=np.asarray(mix, np.float64).reshape(-1, _abi.TW_MIX_REC)), self.device)
+            return Params(_abi.TW_PARAMS_MIXTURE, t["mix"], self.d["prob_gauss_off"])
+        t = _to_device(dict(gauss=np.asarray(gauss, np.float64).reshape(-1, _abi.TW_GAUSS_REC)), self.device)
+        return Params(_abi.TW_PARAMS_GAUSS_BATCHED, t["gauss"], self.d["prob_gauss_off"])
 
     def score(self, params: Params = None, out=None, want_used=False, keep_windows=False):
         """tw_score_topk.  want_used: also emit the candidate maps tw_stitch's fast path needs.
@@ -150,18 +156,11 @@ class Engine:
             out.setdefault("topk_score", torch.empty((n, _abi.TW_K), dtype=torch.float64, device=dev))
             out.setdefault("topk_idx", torch.empty(_abi.TW_K * nt, dtype=torch.int32, device=dev))
             out.setdefault("topk_cnt", torch.empty(n, dtype=torch.uint8, device=dev))
-        s = self._score_struct(out)
-        s.flags = _abi.TW_SCORE_KEEP_WINDOWS if keep_windows else 0
+        s = _abi.fill(_abi.TwScoreOut, out, flags=_abi.TW_SCORE_KEEP_WINDOWS if keep_windows else 0)
         ps = params.struct() if params is not None else None
         _lib.check(self.lib.tw_score_topk(self.h, C.byref(ps) if ps is not None else None, C.byref(s),
                                           self.stream), "tw_score_topk")
         return out
-
-    @staticmethod
-    def _score_struct(out):
-        return _abi.TwScoreOut(_p(out.get("topk_score")), _p(out.get("topk_idx")), _p(out.get("topk_cnt")),
-                               _p(out.get("n_feasible")), _p(out.get("cut")), _p(out.get("used_lo")),
-                               _p(out.get("used_bits")), _p(out.get("used_wide")))
 
     def stitch(self, params: Params, cut, want_topk=False, out=None, undeleted=None):
         """tw_stitch.  undeleted: result of score(params, want_used=True) with the SAME params; lets
@@ -178,10 +177,9 @@ class Engine:
             out.setdefault("topk_score", torch.empty((n, _abi.TW_K), dtype=torch.float64, device=dev))
             out.setdefault("topk_idx", torch.empty(_abi.TW_K * nt, dtype=torch.int32, device=dev))
             out.setdefault("topk_cnt", torch.empty(n, dtype=torch.uint8, device=dev))
-        s = _abi.TwPassOut(_p(out["assign"]), _p(out["mis_rank"]), _p(out["n_cand"]), _p(out.get("topk_score")),
-                           _p(out.get("topk_idx")), _p(out.get("topk_cnt")), _p(out["counters"]))
+        s = _abi.fill(_abi.TwPassOut, out)
         ps = params.struct()
-        und = self._score_struct(undeleted) if undeleted is not None else None
+        und = _abi.fill(_abi.TwScoreOut, undeleted) if undeleted is not None else None
         _lib.check(self.lib.tw_stitch(self.h, C.byref(ps), _p(cut), C.byref(und) if und is not None else None,
                                       C.byref(s), self.stream), "tw_stitch")
         return out

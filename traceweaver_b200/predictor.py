@@ -9,11 +9,10 @@ INTEGRATION.md).  All compute is in the CUDA engine behind the C ABI; this file 
 `Span` objects to SoA arrays and index results back to span ids.
 """
 import numpy as np
-import torch
 
 from . import _abi, refit, skipmode
 from .batch import Problem, build_batch
-from .engine import Engine
+from .engine import Engine, _to_device
 
 METHOD = "MaxScoreBatchSubsetWithSkips"
 NA = ("NA", "NA")
@@ -97,19 +96,44 @@ class TraceWeaverV3:
         d = np.fromiter((sp.duration_mus for sp in spans), np.int64, len(spans))
         return s, s + d
 
-    def _problem(self, process, in_spans, out_span_partitions, invocation_graph):
+    def _marshal(self, process, in_spans, partitions, invocation_graph, fractional):
+        """The Problem of one service solved on `partitions` (the outgoing lists in the order the regime
+        solves them on), the topological callee order and the span ids (in_ids, out_ids per callee)."""
         import networkx as nx
         out_eps = list(nx.topological_sort(invocation_graph))            # traceweaver_v1.py:37-39
-        if set(out_eps) != set(out_span_partitions.keys()):
+        if set(out_eps) != set(partitions.keys()):
             raise ValueError("invocation_graph nodes must be the outgoing endpoints")
         pos = {ep: i for i, ep in enumerate(out_eps)}
-        frac = self._fractional(in_spans) or any(self._fractional(p) for p in out_span_partitions.values())
-        in_s, in_e = self._arrays(in_spans, frac)
-        outs = [self._arrays(out_span_partitions[ep], frac) for ep in out_eps]
+        in_s, in_e = self._arrays(in_spans, fractional)
+        outs = [self._arrays(partitions[ep], fractional) for ep in out_eps]
         preds = [[pos[b] for b, _ in invocation_graph.in_edges(ep)] for ep in out_eps]
         prob = Problem(in_start=in_s, in_end=in_e, out_start=[o[0] for o in outs], out_end=[o[1] for o in outs],
                        preds=preds, name=process)
-        return prob, out_eps
+        in_ids = [s.GetId() for s in in_spans]
+        out_ids = [[s.GetId() for s in partitions[ep]] for ep in out_eps]
+        return prob, out_eps, in_ids, out_ids
+
+    @staticmethod
+    def _result(in_ids, out_eps, out_ids, assign, topk_idx, topk_cnt, n_cand, counters, given_eps,
+                true_assignments):
+        """The reference's 6-tuple (traceweaver_v3.py:1229) from index results: assign [E, n] and
+        topk_idx [n, K, E] hold positions in the lists of `out_ids`, -1 for ("NA", "NA") and, in the
+        skip regime only, <= -2 for ("Skip", "Skip") (traceweaver_v1.py:446-453)."""
+        n = len(in_ids)
+
+        def name(e, c):
+            return out_ids[e][c] if c >= 0 else (NA if c == -1 else SKIP)
+        all_assignments = {ep: {in_ids[i]: name(e, int(assign[e, i])) for i in range(n)} for e, ep in enumerate(out_eps)}
+        all_topk = {ep: {in_ids[i]: [name(e, int(topk_idx[i, r, e])) for r in range(topk_cnt[i])] for i in range(n)}
+                    for e, ep in enumerate(out_eps)}
+        per_span_candidates = {}
+        for ep in given_eps:                                             # traceweaver_v3.py:1096-1098
+            for key in (true_assignments.get(ep, {}) if true_assignments else {}):
+                per_span_candidates[key] = 0
+        for i in range(n):
+            if n_cand[i] or in_ids[i] in per_span_candidates:
+                per_span_candidates[in_ids[i]] = int(n_cand[i])
+        return (all_assignments, all_topk, int(counters[0, 0]), n, per_span_candidates, int(counters[0, 1]))
 
     # -- the reference's entry point ---------------------------------------------------------------
     def FindAssignments(self, method, process, in_span_partitions, out_span_partitions, parallel,
@@ -123,24 +147,32 @@ class TraceWeaverV3:
         in_ep, in_spans = list(in_span_partitions.items())[0]
         # TallySkipSpans re-sorts every partition by start (stable), traceweaver_v3.py:968-971
         in_spans = sorted(in_spans, key=lambda x: float(x.start_mus))
+        frac = self._fractional(in_spans) or any(self._fractional(p) for p in out_span_partitions.values())
         if any(len(p) != len(in_spans) for p in out_span_partitions.values()):
             # skip budgets (cache hits / dynamism): ONE iteration with skip spans, traceweaver_v3.py:1138-1158
-            if self._fractional(in_spans) or any(self._fractional(p) for p in out_span_partitions.values()):
+            if frac:
                 raise NotImplementedError("fractional start_mus (time-compressed spans) on a service with skip "
                                           "budgets: the skip regime keeps int64 timestamps; use the reference")
             if self.carry_state and self._fractional_state:
                 raise NotImplementedError("a service with skip budgets after a service with fractional start_mus: "
                                           "the skip regime would read state built from fractional timestamps; "
                                           "use carry_state=False or the reference")
-            return self._find_assignments_skip(process, in_ep, in_spans, out_span_partitions, true_assignments,
-                                               invocation_graph)
+            # the caller's list order: skipmode.solve sorts the lists itself and names results in this order
+            prob, out_eps, in_ids, out_ids = self._marshal(process, in_spans, out_span_partitions, invocation_graph,
+                                                           frac)
+            state = self.skip_state if self.carry_state else skipmode.SkipState()
+            for a in self._pending_dist:              # BuildDistributions of the earlier services, in call order
+                skipmode.build_distributions(self.engine, *a[:4], a[4], state)
+            self._pending_dist = []
+            res = skipmode.solve(self.engine, prob.in_start, prob.in_end, prob.out_start, prob.out_end, prob.preds,
+                                 labels=[in_ep] + out_eps, state=state, want_topk=False)
+            self.last = res
+            return self._result(in_ids, out_eps, out_ids, res["assign"], res["top2_idx"], res["top2_cnt"],
+                                res["n_cand"], res["counters"], out_span_partitions.keys(), true_assignments)
         out_parts = {ep: sorted(p, key=lambda x: float(x.start_mus)) for ep, p in out_span_partitions.items()}
-        prob, out_eps = self._problem(process, in_spans, out_parts, invocation_graph)
+        prob, out_eps, in_ids, out_ids = self._marshal(process, in_spans, out_parts, invocation_graph, frac)
         hb = build_batch([prob])
         n, E = prob.n_in, prob.E
-
-        in_ids = [s.GetId() for s in in_spans]
-        out_ids = [[s.GetId() for s in out_parts[ep]] for ep in out_eps]
         # ground truth only advances the refit's random stream, exactly as in the reference
         truth = np.full((E, n), -1, np.int32)
         for e, ep in enumerate(out_eps):
@@ -155,71 +187,14 @@ class TraceWeaverV3:
             # in this regime they only leave state behind for a later service with skip budgets: the time
             # windows are appended now (a few tuples), the distribution samples are derived lazily — the
             # arrays are parked and run through tw_build_dist_samples, in call order, when a service with
-            # skip budgets actually arrives (_find_assignments_skip)
+            # skip budgets actually arrives
             self._fractional_state |= hb.float_times
             self.skip_state.time_windows.extend(skipmode.new_time_windows(prob.in_start, prob.in_end))
             self._pending_dist.append((prob.in_start, prob.in_end, prob.out_start, prob.out_end, [in_ep] + out_eps))
-        dev = self.engine.device
         res = solve_batch(self.engine, hb, seed_select=self.seed_select,
-                          truth_assign=torch.from_numpy(truth.reshape(-1)).to(dev),
-                          term_order=torch.from_numpy(order).to(dev))
+                          **_to_device(dict(truth_assign=truth.reshape(-1), term_order=order), self.engine.device))
         self.last = res
-        assign = res["assign"].cpu().numpy().reshape(E, n)
-        topk_idx = res["topk_idx"].cpu().numpy().reshape(n, _abi.TW_K, E)
-        topk_cnt = res["topk_cnt"].cpu().numpy()
-        n_cand = res["n_cand"].cpu().numpy()
-        counters = res["counters"].cpu().numpy()
-
-        all_assignments, all_topk = {}, {}
-        for e, ep in enumerate(out_eps):
-            ids = out_ids[e]
-            col = assign[e]
-            all_assignments[ep] = {in_ids[i]: (ids[col[i]] if col[i] >= 0 else NA) for i in range(n)}
-            all_topk[ep] = {in_ids[i]: [ids[topk_idx[i, r, e]] for r in range(topk_cnt[i])] for i in range(n)}
-        per_span_candidates = {}
-        for ep in out_span_partitions.keys():                            # traceweaver_v3.py:1096-1098
-            for key in (true_assignments.get(ep, {}) if true_assignments else {}):
-                per_span_candidates[key] = 0
-        for i in range(n):
-            if n_cand[i] or in_ids[i] in per_span_candidates:
-                per_span_candidates[in_ids[i]] = int(n_cand[i])
-        return (all_assignments, all_topk, int(counters[0, 0]), n, per_span_candidates, int(counters[0, 1]))
-
-    # -- skip / cache mode (SURVEY.md §8 row f-4) --------------------------------------------------
-    def _find_assignments_skip(self, process, in_ep, in_spans, out_span_partitions, true_assignments,
-                               invocation_graph):
-        import networkx as nx
-        out_eps = list(nx.topological_sort(invocation_graph))            # traceweaver_v1.py:37-39
-        if set(out_eps) != set(out_span_partitions.keys()):
-            raise ValueError("invocation_graph nodes must be the outgoing endpoints")
-        pos = {ep: i for i, ep in enumerate(out_eps)}
-        in_s, in_e = self._arrays(in_spans)
-        outs = [self._arrays(out_span_partitions[ep]) for ep in out_eps]     # the caller's list order
-        preds = [[pos[b] for b, _ in invocation_graph.in_edges(ep)] for ep in out_eps]
-        state = self.skip_state if self.carry_state else skipmode.SkipState()
-        for a in self._pending_dist:                  # BuildDistributions of the earlier services, in call order
-            skipmode.build_distributions(self.engine, *a[:4], a[4], state)
-        self._pending_dist = []
-        res = skipmode.solve(self.engine, in_s, in_e, [o[0] for o in outs], [o[1] for o in outs], preds,
-                             labels=[in_ep] + out_eps, state=state, want_topk=False)
-        self.last = res
-        n, E = len(in_spans), len(out_eps)
-        in_ids = [s.GetId() for s in in_spans]
-        out_ids = [[s.GetId() for s in out_span_partitions[ep]] for ep in out_eps]
-
-        def name(e, c):
-            return out_ids[e][c] if c >= 0 else (NA if c == -1 else SKIP)    # traceweaver_v1.py:446-453
-        assign, top2, cnt = res["assign"], res["top2_idx"], res["top2_cnt"]
-        all_assignments = {ep: {in_ids[i]: name(e, int(assign[e, i])) for i in range(n)} for e, ep in enumerate(out_eps)}
-        all_topk = {ep: {in_ids[i]: [name(e, int(top2[i, r, e])) for r in range(cnt[i])] for i in range(n)}
-                    for e, ep in enumerate(out_eps)}
-        per_span_candidates = {}
-        for ep in out_span_partitions.keys():                            # traceweaver_v3.py:1096-1098
-            for key in (true_assignments.get(ep, {}) if true_assignments else {}):
-                per_span_candidates[key] = 0
-        n_cand = res["n_cand"]
-        for i in range(n):
-            if n_cand[i] or in_ids[i] in per_span_candidates:
-                per_span_candidates[in_ids[i]] = int(n_cand[i])
-        ctr = res["counters"]
-        return (all_assignments, all_topk, int(ctr[0, 0]), n, per_span_candidates, int(ctr[0, 1]))
+        host = {k: res[k].cpu().numpy() for k in ("assign", "topk_idx", "topk_cnt", "n_cand", "counters")}
+        return self._result(in_ids, out_eps, out_ids, host["assign"].reshape(E, n),
+                            host["topk_idx"].reshape(n, _abi.TW_K, E), host["topk_cnt"], host["n_cand"],
+                            host["counters"], out_span_partitions.keys(), true_assignments)

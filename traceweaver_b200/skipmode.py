@@ -20,6 +20,7 @@ import torch
 
 from . import _abi, _lib
 from .batch import Problem, batch_struct, build_batch
+from .engine import _p, _to_device
 
 MAX_WINDOW = _abi.TW_MAX_WINDOW
 
@@ -108,13 +109,12 @@ def build_distributions(engine, in_start, in_end, sorted_out_start, sorted_out_e
     starts, ends, lab = starts[order], ends[order], lab[order]
     large_delay = int(np.max(np.asarray(in_end, np.int64) - np.asarray(in_start, np.int64)))
     dev = engine.device
-    d_s, d_e, d_l = (torch.from_numpy(np.ascontiguousarray(a)).to(dev) for a in (starts, ends, lab))
+    d = _to_device(dict(start=starts, end=ends, label=lab), dev)
     key = torch.empty(len(starts), dtype=torch.int32, device=dev)
     val = torch.empty(len(starts), dtype=torch.int64, device=dev)
-    _lib.check(engine.lib.tw_build_dist_samples(engine.h, len(starts), C.c_void_p(d_s.data_ptr()),
-                                                C.c_void_p(d_e.data_ptr()), C.c_void_p(d_l.data_ptr()), E,
-                                                C.c_int64(large_delay), C.c_void_p(key.data_ptr()),
-                                                C.c_void_p(val.data_ptr()), engine.stream), "tw_build_dist_samples")
+    _lib.check(engine.lib.tw_build_dist_samples(engine.h, len(starts), _p(d["start"]), _p(d["end"]), _p(d["label"]),
+                                                E, C.c_int64(large_delay), _p(key), _p(val), engine.stream),
+               "tw_build_dist_samples")
     key, val = key.cpu().numpy(), val.cpu().numpy()
     dv = state.distribution_values
     for k in np.unique(key[key >= 0]):
@@ -193,13 +193,9 @@ def solve(engine, in_start, in_end, out_start, out_end, preds, labels=None, stat
     hb, host = marshal(in_start, in_end, s_start, s_end, order, preds, wins, counts, pair, budgets)
     dev = engine.device
     n, nt = len(in_start), len(in_start) * E
-
-    def up(a):
-        return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
-
-    d = {k: up(v) for k, v in host.items()}
-    db = {k: up(v.view(np.int32) if v.dtype == np.uint32 else v) for k, v in hb.arrays.items()}
-    sd = _abi.TwSkipDesc(*[C.c_void_p(d[f].data_ptr()) for f, _ in _abi.TwSkipDesc._fields_])
+    d = _to_device(host, dev)
+    db = _to_device(hb.arrays, dev)
+    sd = _abi.fill(_abi.TwSkipDesc, d)
     out = dict(assign=torch.empty(nt, dtype=torch.int32, device=dev), mis_rank=torch.empty(n, dtype=torch.int8, device=dev),
                n_cand=torch.empty(n, dtype=torch.int32, device=dev), counters=torch.zeros((1, 4), dtype=torch.int32, device=dev),
                top2_score=torch.empty((n, _abi.TW_K), dtype=torch.float64, device=dev),
@@ -209,12 +205,7 @@ def solve(engine, in_start, in_end, out_start, out_end, preds, labels=None, stat
         out.update(topk_score=torch.empty((n, _abi.TW_K), dtype=torch.float64, device=dev),
                    topk_idx=torch.empty(_abi.TW_K * nt, dtype=torch.int32, device=dev),
                    topk_cnt=torch.empty(n, dtype=torch.uint8, device=dev))
-
-    def ptr(name):
-        return C.c_void_p(out[name].data_ptr()) if name in out else None
-    so = _abi.TwSkipOut(_abi.TwPassOut(ptr("assign"), ptr("mis_rank"), ptr("n_cand"), ptr("topk_score"), ptr("topk_idx"),
-                                       ptr("topk_cnt"), ptr("counters")),
-                        ptr("top2_score"), ptr("top2_idx"), ptr("top2_cnt"), ptr("cut"))
+    so = _abi.fill(_abi.TwSkipOut, out)
     dev_struct = batch_struct(hb, lambda name: db[name].data_ptr())
     host_struct = batch_struct(hb, lambda name: hb.arrays[name].ctypes.data)
     _lib.check(engine.lib.tw_skip_solve(engine.h, C.byref(dev_struct), C.byref(host_struct), C.byref(sd), C.byref(so),

@@ -8,10 +8,8 @@ import numpy as np
 import torch
 
 from . import _abi, _lib
-
-
-def _p(t):
-    return None if t is None else C.c_void_p(t.data_ptr())
+from .batch import batch_struct, offset_tables
+from .engine import _p, _to_device
 
 
 class TraceLists:
@@ -20,14 +18,8 @@ class TraceLists:
     out_start=[per callee], out_end=[...]); in_trace[p]: int32 [n_in]; out_trace[p]: per callee int32."""
 
     def __init__(self, probs, in_trace, out_trace, n_traces):
-        P = len(probs)
-        n_in = np.array([len(q["in_start"]) for q in probs], np.int64)
-        E = np.array([len(q["out_start"]) for q in probs], np.int64)
-        n_out = [len(o) for q in probs for o in q["out_start"]]
-        a = dict(prob_in_off=np.concatenate([[0], np.cumsum(n_in)]).astype(np.int64),
-                 prob_ep_off=np.concatenate([[0], np.cumsum(E)]).astype(np.int32),
-                 prob_tuple_off=np.concatenate([[0], np.cumsum(n_in * E)]).astype(np.int64),
-                 ep_out_off=np.concatenate([[0], np.cumsum(n_out)]).astype(np.int64))
+        a = offset_tables([len(q["in_start"]) for q in probs], [len(q["out_start"]) for q in probs],
+                          [len(o) for q in probs for o in q["out_start"]])
         cat = lambda xs, dt: np.ascontiguousarray(np.concatenate(xs) if xs else np.zeros(0, dt), dt)
         a["in_start"] = cat([q["in_start"] for q in probs], np.int64)
         a["in_end"] = cat([q["in_end"] for q in probs], np.int64)
@@ -40,7 +32,7 @@ class TraceLists:
         a["prob_trace_lo"] = lo
         a["prob_trace_n"] = (hi - lo + 1).astype(np.int32)
         self.arrays = a
-        self.n_problems = P
+        self.n_problems = len(probs)
         self.n_traces = int(n_traces)
         self.d = None
 
@@ -59,42 +51,21 @@ class TraceLists:
 
     def upload(self, device, resident=None):
         if self.d is None:
-            self.d = {}
-            for k, v in self.arrays.items():
-                if v is None:
-                    continue
-                if resident and k in resident:
-                    self.d[k] = resident[k]
-                else:
-                    self.d[k] = torch.from_numpy(np.ascontiguousarray(v)).to(device)
+            self.d = _to_device(self.arrays, device, resident)
         return self.d
-
-    def struct(self, ptr):
-        a = self.arrays
-        s = _abi.TwBatch()
-        s.n_problems = self.n_problems
-        s.n_ep_total = int(a["prob_ep_off"][-1])
-        s.n_term_total = 0
-        s.n_in_total = int(a["prob_in_off"][-1])
-        s.n_out_total = int(a["ep_out_off"][-1])
-        for name in ("prob_in_off", "prob_ep_off", "prob_tuple_off", "ep_out_off", "in_start", "in_end", "out_start",
-                     "out_end"):
-            setattr(s, name, ptr(name))
-        return s
 
 
 def _structs(engine, tl: TraceLists, resident=None):
     d = tl.upload(engine.device, resident)
-    dev = tl.struct(lambda n: d[n].data_ptr())
-    host = tl.struct(lambda n: tl.arrays[n].ctypes.data)
+    dev = batch_struct(tl, lambda n: d[n].data_ptr())
+    host = batch_struct(tl, lambda n: tl.arrays[n].ctypes.data)
     return d, dev, host
 
 
 def ground_truth(engine, tl: TraceLists):
     """truth[tuple_off[p] + e*n_p + i] (device int32): position of in-span i's child in callee e's list."""
     d, dev, host = _structs(engine, tl)
-    keys = _abi.TwTraceKeys(_p(d["in_trace"]), _p(d["out_trace"]), _p(d["prob_trace_lo"]), _p(d["prob_trace_n"]),
-                            tl.n_traces, 0)
+    keys = _abi.fill(_abi.TwTraceKeys, d, n_traces=tl.n_traces)
     truth = torch.empty(int(tl.arrays["prob_tuple_off"][-1]), dtype=torch.int32, device=engine.device)
     _lib.check(engine.lib.tw_ground_truth(engine.h, C.byref(dev), C.byref(host), C.byref(keys),
                                           C.c_void_p(tl.arrays["prob_trace_n"].ctypes.data), _p(truth), engine.stream),
@@ -118,7 +89,7 @@ def accuracy(engine, tl: TraceLists, truth, assign, topk_idx=None, topk_cnt=None
     P = tl.n_problems
     per = torch.empty((P, 2), dtype=torch.int64, device=engine.device)
     e2e = torch.empty(4, dtype=torch.int64, device=engine.device)
-    pf = None if prob_first is None else torch.from_numpy(np.ascontiguousarray(prob_first, np.uint8)).to(engine.device)
+    pf = None if prob_first is None else _to_device(dict(pf=np.asarray(prob_first, np.uint8)), engine.device)["pf"]
     in_trace = d.get("in_trace")
     _lib.check(engine.lib.tw_accuracy(engine.h, C.byref(dev), C.byref(host), _p(truth), _p(assign), _p(topk_idx),
                                       _p(topk_cnt), _p(in_trace), tl.n_traces if in_trace is not None else 0, _p(pf),
