@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define TW_ABI_VERSION 4
+#define TW_ABI_VERSION 5
 
 /* Algorithm constants hard-coded by the reference. */
 #define TW_MAX_E 8             /* engine limit on out-eps per service (shipped data: <= 4)      */
@@ -244,6 +244,32 @@ int tw_score_topk(tw_engine* eng, const tw_params* params, const tw_score_out* o
  */
 int tw_stitch(tw_engine* eng, const tw_params* params, const uint8_t* cut, const tw_score_out* undeleted,
               const tw_pass_out* out, void* stream);
+
+/*
+ * Score a GIVEN assignment of the bound batch (int64 or tw_engine_bind_f64 binds) under `params`
+ * (either mode; pass 0 uses the record of the in-span's 100-span batch).  `assign` has the layout of
+ * tw_pass_out.assign, so an engine result, a ground truth (tw_ground_truth) or any other predictor's
+ * answer can be passed unchanged.  Per in-span i:
+ *   code_out[i]   TW_ASSESS_* below: the lowest code whose condition holds
+ *   score_out[i]  ScoreAssignmentAsPerInvocationGraph (V1:259-361) of the tuple, the same value
+ *                 tw_score_topk / tw_stitch give that tuple; NaN unless code_out[i] == TW_ASSESS_SCORED
+ *   margin_out[i] against `final_topk` (the no-deletion top-K of tw_score_topk under the same params):
+ *                 the tuple is rank 0 -> s0 - s1 (+inf with a single candidate); else score - s0 (<= 0).
+ *                 NaN when the tuple is not scored or the list is empty.  final_topk and margin_out
+ *                 are both NULL or both set; only topk_score / topk_idx / topk_cnt are read.
+ * Per service p: prob_sum_out[p] = sum of its scored in-spans' scores (a fixed summation order: bit
+ * reproducible), prob_count_out[p * TW_ASSESS_NCODES + c] = its in-spans with code c.
+ * For a float64 bind the records are rescaled as for tw_score_topk, so scores are in real units.
+ */
+#define TW_ASSESS_SCORED 0     /* feasible: scored                                                 */
+#define TW_ASSESS_NA 1         /* -1 (("NA", "NA")) at some callee                                 */
+#define TW_ASSESS_RANGE 2      /* an index outside [0, n_out) of its callee's list                 */
+#define TW_ASSESS_CONTAIN 3    /* a chosen span not inside the in-span (V3:328-333)                */
+#define TW_ASSESS_ORDER 4      /* c_b.end > c_e.start for a DAG edge b -> e (V3:335-347)            */
+#define TW_ASSESS_NCODES 5
+int tw_score_assignments(tw_engine* eng, const tw_params* params, const int32_t* assign,
+                         const tw_score_out* final_topk, double* score_out, uint8_t* code_out, double* margin_out,
+                         double* prob_sum_out, int32_t* prob_count_out, void* stream);
 
 /*
  * Delay samples implied by a pass's assignments, per term (ComputeEpPairDistParams5's

@@ -31,6 +31,8 @@ SYMBOLS = {
     "tw_score_topk": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwParams), C.POINTER(_abi.TwScoreOut), C.c_void_p]),
     "tw_stitch": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwParams), C.c_void_p, C.POINTER(_abi.TwScoreOut),
                             C.POINTER(_abi.TwPassOut), C.c_void_p]),
+    "tw_score_assignments": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwParams), C.c_void_p, C.POINTER(_abi.TwScoreOut),
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tw_delays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tw_gmm_refit": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -95,9 +95,21 @@ class BatchSolver:
         edges = sorted(set([0, hb.n_problems] + [int(c) for c in cuts if 0 < c < hb.n_problems]))
         return [(lo, hi, hb.slice(lo, hi)) for lo, hi in zip(edges[:-1], edges[1:])]
 
-    def solve(self, hb: HostBatch, truth_assign=None, term_order=None, want_scores=False, strict=True):
+    def solve(self, hb: HostBatch, truth_assign=None, term_order=None, want_scores=False, strict=True,
+              want_likelihood=False, want_mixtures=False):
         """want_scores: also return out["topk_score"] (float64 [sum n_in, 5]; the reference's 6-tuple
         carries the top-K ids only, traceweaver_v3.py:1229, so the scores stay on the device by default).
+
+        want_likelihood: how confident each choice is.  The final assignment is scored under the refitted
+        mixtures (tw_score_assignments) and compared with the final top-K:
+            out["chosen_score"]   float64 [sum n_in]  log-likelihood of the chosen tuple, NaN if not scored
+            out["chosen_code"]    uint8   [sum n_in]  TW_ASSESS_* (0 scored, 1 unassigned, ...)
+            out["margin"]         float64 [sum n_in]  chosen = rank 0: s0 - s1 (+inf: single candidate),
+                                                      else score - s0 (<= 0); NaN if not scored
+            out["service_loglik"] float64 [P]         sum of the scored in-spans' log-likelihoods
+            out["service_codes"]  int32   [P, 5]      in-spans per code
+        want_mixtures: out["mixtures"] float64 [n_terms, TW_MIX_REC], the refitted delay model (term order of
+        the batch), and out["mixture_off"] int64 [P+1], the first term of every service; score() takes them.
 
         strict=False: a service that runs into a search limit of the engine (TW_ERR_MWIS_LIMIT: more
         than 2 M branch-and-bound nodes in one window) no longer fails the whole call: the other
@@ -123,6 +135,15 @@ class BatchSolver:
             mis_rank=self._out_buf("mis_rank", n_in, torch.int8))
         if want_scores:
             out["topk_score"] = self._out_buf("topk_score", n_in, torch.float64, _abi.TW_K)
+        if want_likelihood:
+            out.update(chosen_score=self._out_buf("chosen_score", n_in, torch.float64),
+                       chosen_code=self._out_buf("chosen_code", n_in, torch.uint8),
+                       margin=self._out_buf("margin", n_in, torch.float64),
+                       service_loglik=self._out_buf("service_loglik", hb.n_problems, torch.float64),
+                       service_codes=self._out_buf("service_codes", hb.n_problems, torch.int32, _abi.TW_ASSESS_NCODES))
+        mixture_off = hb.ep_term_off[hb.prob_ep_off].astype(np.int64)
+        if want_mixtures:
+            out["mixtures"] = self._out_buf("mixtures", int(mixture_off[-1]), torch.float64, _abi.TW_MIX_REC)
         self.last_chunks = len(plan)
         h2d = d2h = 0
         main = torch.cuda.current_stream(dev)
@@ -159,7 +180,8 @@ class BatchSolver:
                             t.record_stream(self._copy_stream)
                             out[name][b0:b1].copy_(t, non_blocking=True)
 
-                res = solve_bound(eng, seed_select=self.seed_select, check=False, after_score=copy_topk, **inputs)
+                res = solve_bound(eng, seed_select=self.seed_select, check=False, after_score=copy_topk,
+                                  want_likelihood=want_likelihood, **inputs)
                 d2h += sum(res[k].numel() * res[k].element_size()
                            for k in ("topk_idx", "topk_cnt") + (("topk_score",) if want_scores else ()))
                 for name, (b0, b1) in (("assign", (t0, t1)), ("n_cand", (i0, i1)), ("counters", (lo, hi)),
@@ -167,6 +189,23 @@ class BatchSolver:
                     t = res[name]
                     out[name][b0:b1].copy_(t, non_blocking=True)  # D2H
                     d2h += t.numel() * t.element_size()
+                extra = []
+                if want_likelihood:
+                    lk = res["likelihood"]
+                    extra += [("chosen_score", lk["score"], i0, i1), ("chosen_code", lk["code"], i0, i1),
+                              ("margin", lk["margin"], i0, i1), ("service_loglik", lk["prob_sum"], lo, hi),
+                              ("service_codes", lk["prob_count"], lo, hi)]
+                if want_mixtures:
+                    extra.append(("mixtures", res["params_pass1"].table, int(mixture_off[lo]), int(mixture_off[hi])))
+                if extra:                                         # D2H on the copy stream, as the top-K lists
+                    ev = torch.cuda.Event()
+                    ev.record(stream)
+                    self._copy_stream.wait_event(ev)
+                    with torch.cuda.stream(self._copy_stream):
+                        for name, t, b0, b1 in extra:
+                            t.record_stream(self._copy_stream)
+                            out[name][b0:b1].copy_(t, non_blocking=True)
+                            d2h += t.numel() * t.element_size()
             used.append((eng, stream))
         self._copy_stream.synchronize()
         limit_hit = False
@@ -181,6 +220,27 @@ class BatchSolver:
             main.wait_stream(stream)
         self.h2d_bytes, self.d2h_bytes = h2d, d2h
         res = {k: v.numpy() for k, v in out.items()}
+        if want_mixtures:
+            res["mixture_off"] = mixture_off
         if not strict:
             res["failed_services"] = np.flatnonzero(res["counters"][:, 3] != 0) if limit_hit else np.zeros(0, np.int64)
         return res
+
+    def score(self, hb: HostBatch, assign, mixtures):
+        """The likelihood of ANY assignment of `hb` (the layout of out["assign"]: an earlier result, the
+        loader's ground truth, another predictor's answer) under mixtures an earlier
+        solve(hb, want_mixtures=True) returned.  Host arrays: score / code [sum n_in] (code TW_ASSESS_*,
+        score NaN unless code 0), service_loglik [P], service_codes [P, TW_ASSESS_NCODES]."""
+        n_tuple, n_terms = int(hb.prob_tuple_off[-1]), int(hb.ep_term_off[-1])
+        assign = np.asarray(assign, np.int32).reshape(-1)
+        mixtures = np.asarray(mixtures, np.float64)
+        if assign.shape != (n_tuple,) or mixtures.shape != (n_terms, _abi.TW_MIX_REC):
+            raise ValueError(f"score: assign must have {n_tuple} entries and mixtures shape ({n_terms}, "
+                             f"{_abi.TW_MIX_REC}) for this batch")
+        eng = self.engine
+        eng.bind(hb)
+        prm = eng.params_from_host(mix=mixtures)
+        lk = eng.score_assignments(prm, _to_device(dict(assign=assign), eng.device)["assign"])
+        eng.status()
+        return dict(score=lk["score"].cpu().numpy(), code=lk["code"].cpu().numpy(),
+                    service_loglik=lk["prob_sum"].cpu().numpy(), service_codes=lk["prob_count"].cpu().numpy())

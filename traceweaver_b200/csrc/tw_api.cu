@@ -75,6 +75,13 @@ struct tw_engine {
   DevBuf<int32_t> wide_tiles;        // [4*n]: prob, start, scoring-tile index, length
   int n_tiles = 0, n_wide = 0;
   int class_off[TW_MAX_E + 1] = {0};
+  // tw_score_assignments: first scoring tile of every problem (host list built at bind, uploaded on
+  // first use) and the per-tile partial sums
+  std::vector<int32_t> prob_tile0;
+  bool prob_tile0_uploaded = false;
+  DevBuf<int32_t> assess_tile0;
+  DevBuf<double> assess_tile_sum;
+  DevBuf<int32_t> assess_tile_cnt;
   DevBuf<uint8_t> tile_overflow;
   bool windows_valid = false;        // cut / maps / overflow flags of this batch have been produced
   DevBuf<int32_t> own_used_lo;       // candidate maps when the caller does not ask for them
@@ -251,12 +258,15 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
   eng->max_seg = 0;
   eng->windows_valid = false;
   eng->class_off[0] = 0;
+  eng->prob_tile0.assign((size_t)P, 0);
+  eng->prob_tile0_uploaded = false;
   for (int Ec = 1; Ec <= TW_MAX_E; ++Ec) {
     for (int p = 0; p < P; ++p) {
       if (h->prob_ep_off[p + 1] - h->prob_ep_off[p] != Ec) continue;
       int n = (int)(h->prob_in_off[p + 1] - h->prob_in_off[p]);
       for (int i0 = 0; i0 < n; i0 += kS3Tile) {
         int tile_id = (int)nt_prob.size();
+        if (i0 == 0) eng->prob_tile0[p] = tile_id;
         nt_prob.push_back(p);
         nt_start.push_back(i0);
         int lim = i0 + kS3Tile < n ? i0 + kS3Tile : n;
@@ -713,6 +723,40 @@ int tw_stitch(tw_engine* eng, const tw_params* params, const uint8_t* cut, const
   StitchUnits ub{eng->unit_prob.p, eng->unit_lo.p, eng->unit_hi.p, eng->unit_count.p};
   CU(launch_stitch(eng->dev, sp, cut, spec, *out, eng->taken.p, eng->taken_words, eng->node_limit, ub,
                    eng->max_units, eng->stitch_layout, eng->stitch_tables.p, eng->err_flag.p, (cudaStream_t)stream,
+                   eng->launches));
+  return TW_OK;
+}
+
+int tw_score_assignments(tw_engine* eng, const tw_params* params, const int32_t* assign, const tw_score_out* final_topk,
+                         double* score_out, uint8_t* code_out, double* margin_out, double* prob_sum_out,
+                         int32_t* prob_count_out, void* stream) {
+  int rc = need_bound(eng, "tw_score_assignments");
+  if (rc) return rc;
+  if (!params || !assign || !score_out || !code_out || !prob_sum_out || !prob_count_out)
+    return fail(TW_ERR_INVALID, "tw_score_assignments: params, assign, score, code and the per-service outputs are required");
+  if ((final_topk != nullptr) != (margin_out != nullptr))
+    return fail(TW_ERR_INVALID, "tw_score_assignments: final_topk and margin_out go together");
+  if (final_topk && (!final_topk->topk_score || !final_topk->topk_idx || !final_topk->topk_cnt))
+    return fail(TW_ERR_INVALID, "tw_score_assignments: final_topk needs topk_score, topk_idx and topk_cnt");
+  if (params->mode == TW_PARAMS_GAUSS_BATCHED ? (!params->prob_gauss_off || !params->gauss)
+                                              : (params->mode != TW_PARAMS_MIXTURE || !params->mix))
+    return fail(TW_ERR_INVALID, "tw_score_assignments: bad params");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int P = eng->dev.n_problems;
+  if (!eng->prob_tile0_uploaded) {
+    CU(eng->assess_tile0.reserve((size_t)P));
+    CU(cudaMemcpyAsync(eng->assess_tile0.p, eng->prob_tile0.data(), (size_t)P * sizeof(int32_t),
+                       cudaMemcpyHostToDevice, s));
+    eng->prob_tile0_uploaded = true;
+  }
+  CU(eng->assess_tile_sum.reserve((size_t)eng->n_tiles));
+  CU(eng->assess_tile_cnt.reserve((size_t)eng->n_tiles * TW_ASSESS_NCODES));
+  tw_params sp;
+  rc = scoring_params(eng, params, sp, s);
+  if (rc) return rc;
+  AssessOut ao{score_out, code_out, margin_out, prob_sum_out, prob_count_out};
+  CU(launch_assess(eng->dev, sp, assign, final_topk, ao, eng->score_tiles.p, eng->score_tiles.p + eng->n_tiles,
+                   eng->n_tiles, eng->assess_tile0.p, eng->assess_tile_sum.p, eng->assess_tile_cnt.p, s,
                    eng->launches));
   return TW_OK;
 }

@@ -276,6 +276,58 @@ TW_HD double score_tuple(const ProbView& v, const ParamView& pv, int64_t in_s, i
 }
 
 // ---------------------------------------------------------------------------------------------
+// A GIVEN tuple of in-span i (tw_score_assignments): feasibility code, score, margin.
+// `assign` is the batch's tw_pass_out.assign array; tks / tki (NULL: no margin) are the in-span's
+// row of a final top-K list (score[K], idx[K][E]) holding tk_cnt entries.
+// ---------------------------------------------------------------------------------------------
+struct Assessment {
+  double score;
+  double margin;
+  int code;
+};
+
+TW_HD Assessment assess_in_span(const ProbView& v, const ParamView& pv, int i, const int32_t* assign,
+                                const double* tks, const int32_t* tki, int tk_cnt) {
+  Assessment a{NAN, NAN, TW_ASSESS_SCORED};
+  int c[TW_MAX_E];
+  bool na = false, range = false;
+  for (int e = 0; e < v.E; ++e) {
+    c[e] = assign[v.tuple_off + (int64_t)e * v.n_in + i];
+    if (c[e] == -1) na = true;
+    else if (c[e] < 0 || c[e] >= v.n_out[e]) range = true;
+  }
+  if (na || range) {
+    a.code = na ? TW_ASSESS_NA : TW_ASSESS_RANGE;
+    return a;
+  }
+  const int64_t in_s = v.is[i], in_e = v.ie[i];
+  int64_t cs[TW_MAX_E] = {}, ce[TW_MAX_E] = {};
+  bool inside = true;
+  for (int e = 0; e < v.E; ++e) {
+    cs[e] = v.os[e][c[e]];
+    ce[e] = v.oe[e][c[e]];
+    if (cs[e] < in_s || ce[e] > in_e) inside = false;              // V3:328-333
+  }
+  if (!inside) {
+    a.code = TW_ASSESS_CONTAIN;
+    return a;
+  }
+  for (int e = 0; e < v.E; ++e)                                      // V3:335-347: every DAG edge
+    for (int b = 0; b < e; ++b)
+      if ((v.pred[e] >> b & 1u) && ce[b] > cs[e]) {
+        a.code = TW_ASSESS_ORDER;
+        return a;
+      }
+  a.score = score_tuple(v, pv, in_s, in_e, cs, ce);
+  if (tks && tk_cnt > 0) {
+    bool top = true;
+    for (int e = 0; e < v.E; ++e) top = top && tki[e] == c[e];
+    a.margin = !top ? dsub(a.score, tks[0]) : tk_cnt > 1 ? dsub(tks[0], tks[1]) : INFINITY;
+  }
+  return a;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Top-K list: V3:305-307 keeps the K largest (score, stack); V3:461 sorts descending.  Order:
 // score, then the first tuple position whose span differs decides by start (spans.py:51).
 // ---------------------------------------------------------------------------------------------

@@ -115,6 +115,20 @@ cudaError_t launch_params0(const tw_batch& b, const int64_t* in_end_sorted,
                            const int64_t* out_end_sorted, const int64_t* prob_gauss_off,
                            const int32_t* batch_prob, const int32_t* batch_idx, int n_batches_total,
                            double* gauss_out, const int32_t* prob_shift, cudaStream_t s, int64_t& launches);
+// tw_assess.cu: one CTA per scoring tile scores the tile's given tuples and writes per-tile partial sums
+// (tile_sum[t], tile_cnt[t][TW_ASSESS_NCODES]); a second kernel adds them up per service.  `top` may be
+// NULL (no margin).  prob_tile0[p] = first scoring tile of problem p (its tiles are consecutive).
+struct AssessOut {
+  double* score;
+  uint8_t* code;
+  double* margin;
+  double* prob_sum;
+  int32_t* prob_count;
+};
+cudaError_t launch_assess(const tw_batch& b, const tw_params& prm, const int32_t* assign, const tw_score_out* top,
+                          const AssessOut& out, const int32_t* tile_prob, const int32_t* tile_start, int n_tiles,
+                          const int32_t* prob_tile0, double* tile_sum, int32_t* tile_cnt, cudaStream_t s,
+                          int64_t& launches);
 cudaError_t launch_delays(const tw_batch& b, const int32_t* assign, const int64_t* term_sample_off,
                           const int32_t* term_ep, const int32_t* ep_prob, double* delays,
                           int32_t* counts, const int32_t* prob_shift, cudaStream_t s, int64_t& launches);

@@ -184,6 +184,27 @@ class Engine:
                                       C.byref(s), self.stream), "tw_stitch")
         return out
 
+    def score_assignments(self, params: Params, assign, final_topk=None):
+        """tw_score_assignments: the likelihood of a given assignment (tw_pass_out.assign layout, device
+        int32) under `params`.  Device tensors: score / code [n_in] (code: TW_ASSESS_*, score NaN unless
+        code 0), prob_sum [P] (sum of the scored in-spans' scores per service), prob_count [P,
+        TW_ASSESS_NCODES]; with `final_topk` (a score() result under the same params) also margin [n_in]."""
+        dev, n, P = self.device, self.n_in, self.hb.n_problems
+        out = dict(score=torch.empty(n, dtype=torch.float64, device=dev),
+                   code=torch.empty(n, dtype=torch.uint8, device=dev),
+                   prob_sum=torch.empty(P, dtype=torch.float64, device=dev),
+                   prob_count=torch.empty((P, _abi.TW_ASSESS_NCODES), dtype=torch.int32, device=dev))
+        top = None
+        if final_topk is not None:
+            out["margin"] = torch.empty(n, dtype=torch.float64, device=dev)
+            top = _abi.fill(_abi.TwScoreOut, {k: final_topk[k] for k in ("topk_score", "topk_idx", "topk_cnt")})
+        ps = params.struct()
+        _lib.check(self.lib.tw_score_assignments(self.h, C.byref(ps), _p(assign), C.byref(top) if top is not None else None,
+                                                 _p(out["score"]), _p(out["code"]), _p(out.get("margin")),
+                                                 _p(out["prob_sum"]), _p(out["prob_count"]), self.stream),
+                   "tw_score_assignments")
+        return out
+
     def gmm_refit(self, delays, counts, seed_select=10, prob_base_skip=None, term_order=None, want_selected=False):
         """tw_gmm_refit: BIC-selected 1-D GMM per term on the device -> mixture Params."""
         nt = int(self.hb.ep_term_off[-1])

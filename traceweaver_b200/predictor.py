@@ -29,11 +29,14 @@ def solve_batch(eng: Engine, hb, seed_select=10, truth_assign=None, term_order=N
     return solve_bound(eng, seed_select, truth_assign, term_order)
 
 
-def solve_bound(eng: Engine, seed_select=10, truth_assign=None, term_order=None, check=True, after_score=None):
+def solve_bound(eng: Engine, seed_select=10, truth_assign=None, term_order=None, check=True, after_score=None,
+                want_likelihood=False):
     """Both passes over the batch currently bound to `eng` (inputs resident in HBM).  check=False
     leaves the one host sync (engine status) to the caller, who must call eng.status().
     `after_score(top)` is called as soon as the final top-K lists are queued (before the last
-    stitch), so a caller can start copying them out while the stitch runs."""
+    stitch), so a caller can start copying them out while the stitch runs.
+    want_likelihood: also score the final assignment under the refitted mixtures against the final
+    top-K (Engine.score_assignments): result["likelihood"]."""
     eng.prepare()                                 # prev-index scan, sorted end times
     p0 = eng.params_pass0()                       # ComputeEpPairDistParams3, every 100-span batch
     # CreateWindows2 (perfect-cut flags) + FindTopKAssignments on the undeleted lists, pass-0 params
@@ -54,11 +57,15 @@ def solve_bound(eng: Engine, seed_select=10, truth_assign=None, term_order=None,
         after_score(top)
     r1 = eng.stitch(p1, sc["cut"], undeleted=top)  # iteration 1
     n_cand = r0["n_cand"] + r1["n_cand"]          # per_span_candidates accumulates over iterations
+    lik = eng.score_assignments(p1, r1["assign"], final_topk=top) if want_likelihood else None
     if check:
         eng.status()
-    return dict(assign=r1["assign"], mis_rank=r1["mis_rank"], counters=r1["counters"], n_cand=n_cand,
-                topk_score=top["topk_score"], topk_idx=top["topk_idx"], topk_cnt=top["topk_cnt"],
-                cut=sc["cut"], params_pass1=p1, assign_pass0=r0["assign"])
+    res = dict(assign=r1["assign"], mis_rank=r1["mis_rank"], counters=r1["counters"], n_cand=n_cand,
+               topk_score=top["topk_score"], topk_idx=top["topk_idx"], topk_cnt=top["topk_cnt"],
+               cut=sc["cut"], params_pass1=p1, assign_pass0=r0["assign"])
+    if want_likelihood:
+        res["likelihood"] = lik
+    return res
 
 
 class TraceWeaverV3:
