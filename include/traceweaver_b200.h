@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define TW_ABI_VERSION 5
+#define TW_ABI_VERSION 6
 
 /* Algorithm constants hard-coded by the reference. */
 #define TW_MAX_E 8             /* engine limit on out-eps per service (shipped data: <= 4)      */
@@ -272,6 +272,24 @@ int tw_score_assignments(tw_engine* eng, const tw_params* params, const int32_t*
                          double* prob_sum_out, int32_t* prob_count_out, void* stream);
 
 /*
+ * The same for a cache-mode batch (skip budgets): tw_skip_score_assignments, declared with tw_skip_solve
+ * below, takes the batch and descriptor tw_skip_solve takes and does not touch a bound batch.  `assign`
+ * has the layout of tw_pass_out.assign in SORTED-list indices (the indices tw_skip_solve returns):
+ * -1 = ("NA", "NA"), <= -2 = a skip span (which one does not matter: the score does not depend on it).
+ *   code_out[i]   TW_ASSESS_SCORED .. TW_ASSESS_ORDER as above (containment and the DAG order are checked
+ *                 between real spans, as the skip search checks them), else TW_SKIP_ASSESS_UNDEFINED
+ *   score_out[i]  the skip regime's score of the tuple (V1:305-361 with skip spans): the value
+ *                 tw_skip_solve lists for that tuple.  Where some budget is positive it is a MEAN OF
+ *                 DENSITIES (V1:133-136), not a log-likelihood: not comparable with tw_score_assignments.
+ *   margin_out[i] as above, against the in-span's top2 list (top2_score / top2_idx / top2_cnt of a
+ *                 tw_skip_out; the rest of it is not read); two skip spans at one position are equal.
+ * prob_sum_out[p] and prob_count_out[p * TW_SKIP_ASSESS_NCODES + c] as above.
+ */
+#define TW_SKIP_ASSESS_UNDEFINED 5 /* the reference raises on the tuple: all skips, a chain of skipped
+                                      ancestors, or a missing services_times key (V1:264-292, :117-139) */
+#define TW_SKIP_ASSESS_NCODES 6
+
+/*
  * Delay samples implied by a pass's assignments, per term (ComputeEpPairDistParams5's
  * `durations`, traceweaver_v3.py:721-760).  delays[term_sample_off[t] + j]; NA rows are dropped
  * and counts[t] receives the number of samples.  Sample capacity of term t of problem p = n_in_p.
@@ -356,6 +374,13 @@ typedef struct tw_skip_out {
  * arrays as for tw_engine_bind).  Does not touch a batch bound with tw_engine_bind. */
 int tw_skip_solve(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc, const tw_skip_desc* dev_skip,
                   const tw_skip_out* out, void* stream);
+
+/* Score a GIVEN assignment of every problem of `dev` under the model of `dev_skip` (see beside
+ * tw_score_assignments).  top2 and margin_out are both NULL or both set.  Blocks until `stream` is idle. */
+int tw_skip_score_assignments(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc,
+                              const tw_skip_desc* dev_skip, const int32_t* assign, const tw_skip_out* top2,
+                              double* score_out, uint8_t* code_out, double* margin_out, double* prob_sum_out,
+                              int32_t* prob_count_out, void* stream);
 
 /* The parent search of BuildDistributions (v3:120-168) over one service's spans merged by start
  * (stable: incoming spans first, then the out eps in topological order).  label[i]: 0 = incoming

@@ -4,7 +4,7 @@ Field order and widths must match the header exactly; tests/test_abi.py checks s
 against values compiled from the header."""
 import ctypes as C
 
-TW_ABI_VERSION = 5
+TW_ABI_VERSION = 6
 TW_SCORE_KEEP_WINDOWS = 1
 TW_MAX_E = 8
 TW_K = 5
@@ -22,6 +22,8 @@ TW_PARAMS_GAUSS_BATCHED = 0
 TW_PARAMS_MIXTURE = 1
 TW_ASSESS_SCORED, TW_ASSESS_NA, TW_ASSESS_RANGE, TW_ASSESS_CONTAIN, TW_ASSESS_ORDER = 0, 1, 2, 3, 4
 TW_ASSESS_NCODES = 5
+TW_SKIP_ASSESS_UNDEFINED = 5
+TW_SKIP_ASSESS_NCODES = 6
 
 TW_OK = 0
 TW_ERR_INVALID, TW_ERR_CUDA, TW_ERR_MWIS_LIMIT, TW_ERR_RANGE_LIMIT, TW_ERR_UNSUPPORTED, TW_ERR_NO_DEVICE, \

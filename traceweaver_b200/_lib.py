@@ -39,6 +39,9 @@ SYMBOLS = {
     "tw_gmm_stream_draws": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tw_skip_solve": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch),
                                 C.POINTER(_abi.TwSkipDesc), C.POINTER(_abi.TwSkipOut), C.c_void_p]),
+    "tw_skip_score_assignments": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch),
+                                            C.POINTER(_abi.TwSkipDesc), C.c_void_p, C.POINTER(_abi.TwSkipOut),
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tw_gmm_work": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.c_int]),
     "tw_measure_fp64_peak": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_void_p]),
     "tw_ground_truth": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch),

@@ -102,6 +102,9 @@ struct tw_engine {
   DevBuf<int64_t> skip_set_off;
   DevBuf<uint32_t> skip_taken;
   DevBuf<int32_t> skip_win;
+  DevBuf<int32_t> skip_tiles;        // tw_skip_score_assignments: tile prob, tile start, first tile per problem
+  DevBuf<double> skip_tile_sum;      // and the per-tile partials
+  DevBuf<int32_t> skip_tile_cnt;
   DevBuf<int32_t> unit_prob;         // stitch units (k_stitch_units)
   DevBuf<int32_t> unit_lo;
   DevBuf<int32_t> unit_hi;
@@ -518,6 +521,44 @@ int tw_skip_solve(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const 
   CU(launch_skip(*dev, *sd, *out, eng->skip_taken.p, eng->skip_sets.p, eng->skip_set_off.p, eng->skip_win.p,
                  eng->node_limit, eng->err_flag.p, s, eng->launches));
   CU(cudaStreamSynchronize(s));    // set_off goes out of scope
+  return TW_OK;
+}
+
+int tw_skip_score_assignments(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const tw_skip_desc* sd,
+                              const int32_t* assign, const tw_skip_out* top2, double* score_out, uint8_t* code_out,
+                              double* margin_out, double* prob_sum_out, int32_t* prob_count_out, void* stream_) {
+  if (!eng || !dev || !h || !sd || !assign || !score_out || !code_out || !prob_sum_out || !prob_count_out)
+    return fail(TW_ERR_INVALID, "tw_skip_score_assignments: NULL argument");
+  if ((top2 != nullptr) != (margin_out != nullptr))
+    return fail(TW_ERR_INVALID, "tw_skip_score_assignments: top2 and margin_out go together");
+  if (top2 && (!top2->top2_score || !top2->top2_idx || !top2->top2_cnt))
+    return fail(TW_ERR_INVALID, "tw_skip_score_assignments: top2 needs top2_score, top2_idx and top2_cnt");
+  int rc = validate_host(h, "tw_skip_score_assignments", true, true);
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream_;
+  CU(cudaSetDevice(eng->device));
+  // 128-in-span tiles, a service's tiles consecutive: [tile prob | tile start | first tile of every problem]
+  const int P = h->n_problems;
+  std::vector<int32_t> tprob, tstart, tile0((size_t)P);
+  for (int p = 0; p < P; ++p) {
+    tile0[p] = (int32_t)tprob.size();
+    const int64_t n = h->prob_in_off[p + 1] - h->prob_in_off[p];
+    for (int64_t i0 = 0; i0 < n; i0 += kAssessThreads) {
+      tprob.push_back(p);
+      tstart.push_back((int32_t)i0);
+    }
+  }
+  const int nt = (int)tprob.size();
+  tprob.insert(tprob.end(), tstart.begin(), tstart.end());
+  tprob.insert(tprob.end(), tile0.begin(), tile0.end());
+  CU(eng->skip_tiles.reserve(tprob.size()));
+  CU(eng->skip_tile_sum.reserve((size_t)nt));
+  CU(eng->skip_tile_cnt.reserve((size_t)nt * TW_SKIP_ASSESS_NCODES));
+  CU(cudaMemcpyAsync(eng->skip_tiles.p, tprob.data(), tprob.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+  AssessOut ao{score_out, code_out, margin_out, prob_sum_out, prob_count_out};
+  CU(launch_skip_assess(*dev, *sd, assign, top2, ao, eng->skip_tiles.p, eng->skip_tiles.p + nt, nt,
+                        eng->skip_tiles.p + 2 * nt, eng->skip_tile_sum.p, eng->skip_tile_cnt.p, s, eng->launches));
+  CU(cudaStreamSynchronize(s));    // the tile lists go out of scope
   return TW_OK;
 }
 

@@ -7,18 +7,13 @@
 
 namespace tw {
 
-constexpr int kAssessThreads = kS3Tile;          // one CTA per scoring tile, one thread per in-span
-constexpr unsigned kAll = 0xffffffffu;
-
 __global__ void __launch_bounds__(kAssessThreads)
 k_assess(tw_batch b, tw_params prm, const int32_t* __restrict__ assign, tw_score_out top, int with_top,
          AssessOut out, const int32_t* __restrict__ tile_prob, const int32_t* __restrict__ tile_start,
          double* __restrict__ tile_sum, int32_t* __restrict__ tile_cnt) {
   __shared__ double etab[64];
   __shared__ ProbView v;
-  __shared__ double wsum[kAssessThreads / 32];
-  __shared__ int wcnt[kAssessThreads / 32][TW_ASSESS_NCODES];
-  const int t = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int t = blockIdx.x, tid = threadIdx.x;
   const int p = tile_prob[t];
   if (tid == 0) load_view(b, p, v);              // the batch was validated at bind
   load_exp_table(etab);                          // its barrier also publishes v
@@ -44,32 +39,12 @@ k_assess(tw_batch b, tw_params prm, const int32_t* __restrict__ assign, tw_score
     code = a.code;
     if (code == TW_ASSESS_SCORED) sc = a.score;
   }
-  // per-tile partials in a fixed order: butterfly within each warp (every lane ends with the same
-  // bits), then the four warps in order
-#pragma unroll
-  for (int d = 16; d > 0; d >>= 1) sc = dadd(sc, __shfl_xor_sync(kAll, sc, d));
-  int cnt[TW_ASSESS_NCODES];
-#pragma unroll
-  for (int q = 0; q < TW_ASSESS_NCODES; ++q) cnt[q] = __popc(__ballot_sync(kAll, code == q));
-  if (lane == 0) {
-    wsum[wid] = sc;
-#pragma unroll
-    for (int q = 0; q < TW_ASSESS_NCODES; ++q) wcnt[wid][q] = cnt[q];
-  }
-  __syncthreads();
-  if (tid == 0) {
-    double s = wsum[0];
-    for (int w = 1; w < kAssessThreads / 32; ++w) s = dadd(s, wsum[w]);
-    tile_sum[t] = s;
-  }
-  if (tid < TW_ASSESS_NCODES) {
-    int c = 0;
-    for (int w = 0; w < kAssessThreads / 32; ++w) c += wcnt[w][tid];
-    tile_cnt[(size_t)t * TW_ASSESS_NCODES + tid] = c;
-  }
+  assess_tile_partials<TW_ASSESS_NCODES>(sc, code, t, tile_sum, tile_cnt);
 }
 
-// one warp per service: lane l adds tiles l, l + 32, ... in order, then a butterfly
+// one warp per service: lane l adds tiles l, l + 32, ... in order, then a butterfly.  NC: the codes of
+// the assessment kernel whose partials it adds (k_assess, k_skip_assess)
+template <int NC>
 __global__ void __launch_bounds__(128)
 k_assess_reduce(int n_problems, const int64_t* __restrict__ prob_in_off, const int32_t* __restrict__ prob_tile0,
                 const double* __restrict__ tile_sum, const int32_t* __restrict__ tile_cnt,
@@ -79,22 +54,22 @@ k_assess_reduce(int n_problems, const int64_t* __restrict__ prob_in_off, const i
   const int t0 = prob_tile0[p];
   const int nt = (int)((prob_in_off[p + 1] - prob_in_off[p] + kS3Tile - 1) / kS3Tile);
   double s = 0.0;
-  int cnt[TW_ASSESS_NCODES] = {0};
+  int cnt[NC] = {0};
   for (int k = lane; k < nt; k += 32) {
     s = dadd(s, tile_sum[t0 + k]);
 #pragma unroll
-    for (int q = 0; q < TW_ASSESS_NCODES; ++q) cnt[q] += tile_cnt[(size_t)(t0 + k) * TW_ASSESS_NCODES + q];
+    for (int q = 0; q < NC; ++q) cnt[q] += tile_cnt[(size_t)(t0 + k) * NC + q];
   }
 #pragma unroll
   for (int d = 16; d > 0; d >>= 1) {
-    s = dadd(s, __shfl_xor_sync(kAll, s, d));
+    s = dadd(s, __shfl_xor_sync(kAssessAll, s, d));
 #pragma unroll
-    for (int q = 0; q < TW_ASSESS_NCODES; ++q) cnt[q] += __shfl_xor_sync(kAll, cnt[q], d);
+    for (int q = 0; q < NC; ++q) cnt[q] += __shfl_xor_sync(kAssessAll, cnt[q], d);
   }
   if (lane == 0) {
     prob_sum[p] = s;
 #pragma unroll
-    for (int q = 0; q < TW_ASSESS_NCODES; ++q) prob_count[(size_t)p * TW_ASSESS_NCODES + q] = cnt[q];
+    for (int q = 0; q < NC; ++q) prob_count[(size_t)p * NC + q] = cnt[q];
   }
 }
 
@@ -109,10 +84,21 @@ cudaError_t launch_assess(const tw_batch& b, const tw_params& prm, const int32_t
                                               tile_sum, tile_cnt);
   cudaError_t e = after_launch(launches);
   if (e != cudaSuccess) return e;
+  return launch_assess_reduce(TW_ASSESS_NCODES, b.n_problems, b.prob_in_off, prob_tile0, tile_sum, tile_cnt,
+                              out.prob_sum, out.prob_count, s, launches);
+}
+
+cudaError_t launch_assess_reduce(int n_codes, int n_problems, const int64_t* prob_in_off, const int32_t* prob_tile0,
+                                 const double* tile_sum, const int32_t* tile_cnt, double* prob_sum,
+                                 int32_t* prob_count, cudaStream_t s, int64_t& launches) {
   const int warps_per_block = 128 / 32;
-  const int grid = (b.n_problems + warps_per_block - 1) / warps_per_block;
-  k_assess_reduce<<<grid, 128, 0, s>>>(b.n_problems, b.prob_in_off, prob_tile0, tile_sum, tile_cnt, out.prob_sum,
-                                       out.prob_count);
+  const int grid = (n_problems + warps_per_block - 1) / warps_per_block;
+  if (n_codes == TW_ASSESS_NCODES)
+    k_assess_reduce<TW_ASSESS_NCODES><<<grid, 128, 0, s>>>(n_problems, prob_in_off, prob_tile0, tile_sum, tile_cnt,
+                                                           prob_sum, prob_count);
+  else
+    k_assess_reduce<TW_SKIP_ASSESS_NCODES><<<grid, 128, 0, s>>>(n_problems, prob_in_off, prob_tile0, tile_sum,
+                                                                tile_cnt, prob_sum, prob_count);
   return after_launch(launches);
 }
 

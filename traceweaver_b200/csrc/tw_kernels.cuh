@@ -129,6 +129,49 @@ cudaError_t launch_assess(const tw_batch& b, const tw_params& prm, const int32_t
                           const AssessOut& out, const int32_t* tile_prob, const int32_t* tile_start, int n_tiles,
                           const int32_t* prob_tile0, double* tile_sum, int32_t* tile_cnt, cudaStream_t s,
                           int64_t& launches);
+// tw_skip_assess.cu: the same for a cache-mode batch (tw_skip_score_assignments) over its 128-in-span tiles,
+// with TW_SKIP_ASSESS_NCODES codes; `top2` may be NULL (no margin)
+cudaError_t launch_skip_assess(const tw_batch& b, const tw_skip_desc& sd, const int32_t* assign, const tw_skip_out* top2,
+                               const AssessOut& out, const int32_t* tile_prob, const int32_t* tile_start, int n_tiles,
+                               const int32_t* prob_tile0, double* tile_sum, int32_t* tile_cnt, cudaStream_t s,
+                               int64_t& launches);
+// the per-service sums of either kernel's tile partials; n_codes: TW_ASSESS_NCODES or TW_SKIP_ASSESS_NCODES
+cudaError_t launch_assess_reduce(int n_codes, int n_problems, const int64_t* prob_in_off, const int32_t* prob_tile0,
+                                 const double* tile_sum, const int32_t* tile_cnt, double* prob_sum,
+                                 int32_t* prob_count, cudaStream_t s, int64_t& launches);
+constexpr int kAssessThreads = kS3Tile;          // one CTA per 128-in-span tile, one thread per in-span
+constexpr unsigned kAssessAll = 0xffffffffu;
+// Per-tile partials of the assessment kernels: `sc` (0 unless scored) and `code` (-1: no in-span) of every
+// thread -> tile_sum[t], tile_cnt[t][NC].  A fixed order: a butterfly within each warp (every lane ends with
+// the same bits), then the warps in order.
+template <int NC>
+__device__ __forceinline__ void assess_tile_partials(double sc, int code, int t, double* __restrict__ tile_sum,
+                                                     int32_t* __restrict__ tile_cnt) {
+  __shared__ double wsum[kAssessThreads / 32];
+  __shared__ int wcnt[kAssessThreads / 32][NC];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) sc = dadd(sc, __shfl_xor_sync(kAssessAll, sc, d));
+  int cnt[NC];
+#pragma unroll
+  for (int q = 0; q < NC; ++q) cnt[q] = __popc(__ballot_sync(kAssessAll, code == q));
+  if (lane == 0) {
+    wsum[wid] = sc;
+#pragma unroll
+    for (int q = 0; q < NC; ++q) wcnt[wid][q] = cnt[q];
+  }
+  __syncthreads();
+  if (tid == 0) {
+    double s = wsum[0];
+    for (int w = 1; w < kAssessThreads / 32; ++w) s = dadd(s, wsum[w]);
+    tile_sum[t] = s;
+  }
+  if (tid < NC) {
+    int c = 0;
+    for (int w = 0; w < kAssessThreads / 32; ++w) c += wcnt[w][tid];
+    tile_cnt[(size_t)t * NC + tid] = c;
+  }
+}
 cudaError_t launch_delays(const tw_batch& b, const int32_t* assign, const int64_t* term_sample_off,
                           const int32_t* term_ep, const int32_t* ep_prob, double* delays,
                           int32_t* counts, const int32_t* prob_shift, cudaStream_t s, int64_t& launches);

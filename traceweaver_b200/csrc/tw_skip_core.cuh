@@ -39,6 +39,25 @@ struct SkipProb {
   const int32_t* sorted_of_entry[TW_MAX_E];
 };
 
+// The model and lists of problem p as tw_skip_desc describes them.  skip_base / fetches, the search's
+// per-window cursors, are scratch of the caller that searches; they stay NULL here.
+TW_HD SkipProb skip_prob(const tw_skip_desc& sd, const ProbView& v, int p) {
+  SkipProb sp;
+  sp.n_win = (int)(sd.prob_win_off[p + 1] - sd.prob_win_off[p]);
+  sp.win_start = sd.win_start + sd.prob_win_off[p];
+  sp.skip_count = sd.skip_count + sd.prob_cnt_off[p];
+  sp.skip_base = nullptr;
+  sp.fetches = nullptr;
+  sp.pair = sd.pair_gauss + 2 * sd.prob_pair_off[p];
+  sp.normalized = sd.prob_normalized[p];
+  sp.pred_order = sd.ep_pred_order + (size_t)v.ep0 * TW_MAX_E;
+  for (int e = 0; e < v.E; ++e) {
+    sp.entry_pos[e] = sd.out_entry_pos + v.out_off[e];
+    sp.sorted_of_entry[e] = sd.out_sorted_of_entry + v.out_off[e];
+  }
+  return sp;
+}
+
 struct SkipShared {
   WindowBuf wb;
   TopK tk;
@@ -110,6 +129,52 @@ TW_HD_NOINLINE inline double skip_score(const ProbView& v, const SkipProb& sp, i
     if (e == last) { total = dadd(total, pair_cost(sp, E, 1 + e, 0, in_e - ce, undefined)); ++num; }
   }
   return sp.normalized ? ddiv(total, (double)num) : total;
+}
+
+// A GIVEN tuple of in-span i (tw_skip_score_assignments), the skip regime's assess_in_span: `assign` is
+// the batch's tw_pass_out.assign array in sorted-list indices (-1 NA, <= -2 a skip span, whichever);
+// tks / tki (NULL: no margin) are the in-span's row of its top2 list holding tk_cnt entries.  The
+// feasibility checks are the candidate filter and the DAG check skip_topk applies while it builds a
+// tuple, the score is skip_score's, so a listed tuple gets its listed score bit for bit.
+TW_HD_NOINLINE inline Assessment skip_assess_in_span(const ProbView& v, const SkipProb& sp, int i, const int32_t* assign,
+                                     const double* tks, const int32_t* tki, int tk_cnt) {
+  Assessment a{NAN, NAN, TW_ASSESS_SCORED};
+  int c[TW_MAX_E];
+  bool na = false, range = false;
+  for (int e = 0; e < v.E; ++e) {
+    c[e] = assign[v.tuple_off + (int64_t)e * v.n_in + i];
+    if (c[e] == -1) na = true;
+    else if (c[e] >= v.n_out[e]) range = true;
+  }
+  if (na || range) {
+    a.code = na ? TW_ASSESS_NA : TW_ASSESS_RANGE;
+    return a;
+  }
+  const int64_t in_s = v.is[i], in_e = v.ie[i];
+  for (int e = 0; e < v.E; ++e)                                      // V3:328-333
+    if (c[e] >= 0 && (v.os[e][c[e]] < in_s || v.oe[e][c[e]] > in_e)) {
+      a.code = TW_ASSESS_CONTAIN;
+      return a;
+    }
+  for (int e = 0; e < v.E; ++e)                                      // V3:335-347, as skip_topk
+    for (int b = 0; b < e; ++b)
+      if (c[e] >= 0 && (v.pred[e] >> b & 1u) && c[b] >= 0 && v.oe[b][c[b]] > v.os[e][c[e]]) {
+        a.code = TW_ASSESS_ORDER;
+        return a;
+      }
+  bool undefined = false;
+  const double score = skip_score(v, sp, in_s, in_e, c, &undefined);
+  if (undefined) {
+    a.code = TW_SKIP_ASSESS_UNDEFINED;
+    return a;
+  }
+  a.score = score;
+  if (tks && tk_cnt > 0) {
+    bool top = true;                                                 // skips at one position are one span here
+    for (int e = 0; e < v.E; ++e) top = top && (tki[e] == c[e] || (tki[e] < -1 && c[e] < -1));
+    a.margin = !top ? dsub(a.score, tks[0]) : tk_cnt > 1 ? dsub(tks[0], tks[1]) : INFINITY;
+  }
+  return a;
 }
 
 // FetchSkipFromWindow, V3:820-842: the least-used skip span of the in-span's time window, first on ties
@@ -386,22 +451,14 @@ TW_HD_NOINLINE inline int skip_solve_problem(const tw_batch& b, int p, const tw_
   ProbView v;
   if (load_view(b, p, v) != TW_OK) return TW_ERR_INVALID;
   const int E = v.E, n = v.n_in;
-  SkipProb sp;
-  sp.n_win = (int)(sd.prob_win_off[p + 1] - sd.prob_win_off[p]);
-  sp.win_start = sd.win_start + sd.prob_win_off[p];
-  sp.skip_count = sd.skip_count + sd.prob_cnt_off[p];
+  SkipProb sp = skip_prob(sd, v, p);
   sp.skip_base = win_scratch + 2 * sd.prob_cnt_off[p];
   sp.fetches = sp.skip_base + (size_t)E * sp.n_win;
-  sp.pair = sd.pair_gauss + 2 * sd.prob_pair_off[p];
-  sp.normalized = sd.prob_normalized[p];
-  sp.pred_order = sd.ep_pred_order + (size_t)v.ep0 * TW_MAX_E;
   EntryList el[TW_MAX_E];
   int set_off[TW_MAX_E];
   int64_t taken_off[TW_MAX_E];
   int set_bits = 0;
   for (int e = 0; e < E; ++e) {
-    sp.entry_pos[e] = sd.out_entry_pos + v.out_off[e];
-    sp.sorted_of_entry[e] = sd.out_sorted_of_entry + v.out_off[e];
     el[e].s = v.os[e]; el[e].e = v.oe[e]; el[e].of_entry = sp.sorted_of_entry[e]; el[e].n = v.n_out[e];
     set_off[e] = set_bits;
     set_bits += (v.n_out[e] + 31) & ~31;

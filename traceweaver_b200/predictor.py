@@ -20,13 +20,13 @@ SKIP = ("Skip", "Skip")
 
 
 def solve_batch(eng: Engine, hb, seed_select=10, truth_assign=None, term_order=None, device_arrays=None,
-                pinned=False, keep=("assign", "mis_rank", "counters", "n_cand", "topk")):
+                pinned=False, keep=("assign", "mis_rank", "counters", "n_cand", "topk"), want_likelihood=False):
     """The whole path for a bound-able batch: both passes of traceweaver_v3.py:1159-1227.
 
     params0 -> windows -> stitch (pass 0) -> delays -> refit -> score (final top-K) -> stitch
     (pass 1).  Returns device tensors; one host sync at the end (engine status)."""
     eng.bind(hb, device_arrays=device_arrays, pinned=pinned)
-    return solve_bound(eng, seed_select, truth_assign, term_order)
+    return solve_bound(eng, seed_select, truth_assign, term_order, want_likelihood=want_likelihood)
 
 
 def solve_bound(eng: Engine, seed_select=10, truth_assign=None, term_order=None, check=True, after_score=None,
@@ -69,14 +69,27 @@ def solve_bound(eng: Engine, seed_select=10, truth_assign=None, term_order=None,
 
 
 class TraceWeaverV3:
-    """`predictors` entry replacing the reference's ("MaxScoreBatchSubsetWithSkips", TraceWeaverV3)."""
+    """`predictors` entry replacing the reference's ("MaxScoreBatchSubsetWithSkips", TraceWeaverV3).
 
-    def __init__(self, all_spans, all_processes, device=0, seed_select=10, carry_state=True):
+    want_likelihood=True: every FindAssignments call also scores its own final assignment under the model
+    it solved with and leaves `self.last_likelihood`:
+        in_spans       {in-span id: (score, code, margin)}   code TW_ASSESS_* (1 = unassigned), score NaN
+                       unless code 0, margin s0 - s1 (+inf) when the chosen tuple is the best one, else score - s0
+        service_score  sum of the scored in-spans' scores
+        service_codes  in-spans per code
+        regime         "two_pass": scores are log-likelihoods under the refitted mixtures;
+                       "skip" (a service with skip budgets): the skip regime's scores, means of densities
+                       where a budget is positive, so the two are not comparable
+    The 6-tuple is the same either way."""
+
+    def __init__(self, all_spans, all_processes, device=0, seed_select=10, carry_state=True, want_likelihood=False):
         self.all_spans = all_spans
         self.all_processes = all_processes
         self.seed_select = seed_select
         self.engine = Engine(device)          # raises without a CUDA device: there is no CPU path
         self.last = None
+        self.want_likelihood = want_likelihood
+        self.last_likelihood = None
         # what the reference's instance keeps from one service to the next and its skip regime reads
         # (time_windows, distribution_values: traceweaver_v3.py:40,45 are never reset)
         self.skip_state = skipmode.SkipState()
@@ -142,6 +155,11 @@ class TraceWeaverV3:
                 per_span_candidates[in_ids[i]] = int(n_cand[i])
         return (all_assignments, all_topk, int(counters[0, 0]), n, per_span_candidates, int(counters[0, 1]))
 
+    @staticmethod
+    def _likelihood(regime, in_ids, score, code, margin, service_score, service_codes):
+        return dict(in_spans={iid: (float(score[i]), int(code[i]), float(margin[i])) for i, iid in enumerate(in_ids)},
+                    service_score=float(service_score), service_codes=np.asarray(service_codes), regime=regime)
+
     # -- the reference's entry point ---------------------------------------------------------------
     def FindAssignments(self, method, process, in_span_partitions, out_span_partitions, parallel,
                         instrumented_hops, true_assignments, invocation_graph, true_skips=False,
@@ -172,8 +190,12 @@ class TraceWeaverV3:
                 skipmode.build_distributions(self.engine, *a[:4], a[4], state)
             self._pending_dist = []
             res = skipmode.solve(self.engine, prob.in_start, prob.in_end, prob.out_start, prob.out_end, prob.preds,
-                                 labels=[in_ep] + out_eps, state=state, want_topk=False)
+                                 labels=[in_ep] + out_eps, state=state, want_topk=False,
+                                 want_likelihood=self.want_likelihood)
             self.last = res
+            if self.want_likelihood:
+                self.last_likelihood = self._likelihood("skip", in_ids, res["chosen_score"], res["chosen_code"],
+                                                        res["margin"], res["service_score"], res["service_codes"])
             return self._result(in_ids, out_eps, out_ids, res["assign"], res["top2_idx"], res["top2_cnt"],
                                 res["n_cand"], res["counters"], out_span_partitions.keys(), true_assignments)
         out_parts = {ep: sorted(p, key=lambda x: float(x.start_mus)) for ep, p in out_span_partitions.items()}
@@ -198,9 +220,13 @@ class TraceWeaverV3:
             self._fractional_state |= hb.float_times
             self.skip_state.time_windows.extend(skipmode.new_time_windows(prob.in_start, prob.in_end))
             self._pending_dist.append((prob.in_start, prob.in_end, prob.out_start, prob.out_end, [in_ep] + out_eps))
-        res = solve_batch(self.engine, hb, seed_select=self.seed_select,
+        res = solve_batch(self.engine, hb, seed_select=self.seed_select, want_likelihood=self.want_likelihood,
                           **_to_device(dict(truth_assign=truth.reshape(-1), term_order=order), self.engine.device))
         self.last = res
+        if self.want_likelihood:
+            lk = {k: v.cpu().numpy() for k, v in res["likelihood"].items()}
+            self.last_likelihood = self._likelihood("two_pass", in_ids, lk["score"], lk["code"], lk["margin"],
+                                                    lk["prob_sum"][0], lk["prob_count"][0])
         host = {k: res[k].cpu().numpy() for k in ("assign", "topk_idx", "topk_cnt", "n_cand", "counters")}
         return self._result(in_ids, out_eps, out_ids, host["assign"].reshape(E, n),
                             host["topk_idx"].reshape(n, _abi.TW_K, E), host["topk_cnt"], host["n_cand"],

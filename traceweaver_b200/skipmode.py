@@ -176,12 +176,67 @@ def to_caller_order(res, order, n, E, want_topk=True):
     return res
 
 
+def to_sorted_order(idx, order, ep_last):
+    """Inverse of to_caller_order for one index array: positions in the caller's lists -> sorted-list
+    indices.  Codes < 0 stay, and so does a position past the end of its list (scored as out of range)."""
+    idx = np.array(idx, np.int32)
+    for e, od in enumerate(order):
+        col = idx[..., e] if ep_last else idx[e]
+        m = (col >= 0) & (col < len(od))
+        col[m] = np.argsort(od)[col[m]]
+    return idx
+
+
+def _descriptors(engine, hb, host):
+    """Device copies of a marshalled service and the three structs tw_skip_solve and
+    tw_skip_score_assignments take (the device arrays ride along: they must outlive the call)."""
+    d = _to_device(host, engine.device)
+    db = _to_device(hb.arrays, engine.device)
+    return (batch_struct(hb, lambda name: db[name].data_ptr()), batch_struct(hb, lambda name: hb.arrays[name].ctypes.data),
+            _abi.fill(_abi.TwSkipDesc, d), (d, db))
+
+
+def _assess(engine, structs, n, assign, top2=None):
+    """tw_skip_score_assignments of ONE service: device tensors score / code / margin (with `top2`, a
+    TwSkipOut) per in-span, prob_sum [1], prob_count [1, TW_SKIP_ASSESS_NCODES]."""
+    dev_struct, host_struct, sd, _ = structs
+    dev = engine.device
+    lk = dict(score=torch.empty(n, dtype=torch.float64, device=dev), code=torch.empty(n, dtype=torch.uint8, device=dev),
+              prob_sum=torch.empty(1, dtype=torch.float64, device=dev),
+              prob_count=torch.empty((1, _abi.TW_SKIP_ASSESS_NCODES), dtype=torch.int32, device=dev))
+    if top2 is not None:
+        lk["margin"] = torch.empty(n, dtype=torch.float64, device=dev)
+    _lib.check(engine.lib.tw_skip_score_assignments(
+        engine.h, C.byref(dev_struct), C.byref(host_struct), C.byref(sd), _p(assign),
+        C.byref(top2) if top2 is not None else None, _p(lk["score"]), _p(lk["code"]), _p(lk.get("margin")),
+        _p(lk["prob_sum"]), _p(lk["prob_count"]), engine.stream), "tw_skip_score_assignments")
+    return lk
+
+
+def _likelihood(lk):
+    res = dict(chosen_score=lk["score"].cpu().numpy(), chosen_code=lk["code"].cpu().numpy(),
+               service_score=float(lk["prob_sum"][0]), service_codes=lk["prob_count"][0].cpu().numpy())
+    if "margin" in lk:
+        res["margin"] = lk["margin"].cpu().numpy()
+    return res
+
+
 def solve(engine, in_start, in_end, out_start, out_end, preds, labels=None, state: SkipState = None,
-          want_topk=True):
+          want_topk=True, want_likelihood=False):
     """One FindAssignments call in the skip regime for ONE service.  out_start/out_end: per ep
     (topological order) in the CALLER's list order.  Returns numpy arrays; out spans are named by their
     position in the caller's lists, skip spans by -2 - g (see include/traceweaver_b200.h), ("Skip", "Skip")
-    assignments by -2, ("NA", "NA") by -1."""
+    assignments by -2, ("NA", "NA") by -1.
+
+    want_likelihood: also how sure the engine is of each choice.  Its final assignment is scored under the
+    model it solved with (tw_skip_score_assignments) and compared with the in-span's top2 list:
+        chosen_score   float64 [n]  the tuple's score, NaN unless scored.  Where some budget is positive
+                                    (the normal case here) a MEAN OF DENSITIES, not a log-likelihood:
+                                    not comparable with the two-pass regime's scores
+        chosen_code    uint8   [n]  TW_ASSESS_* / TW_SKIP_ASSESS_UNDEFINED (1 = unassigned)
+        margin         float64 [n]  chosen = rank 0: s0 - s1 (+inf: single candidate), else score - s0
+        service_score  float        sum of the scored in-spans' scores
+        service_codes  int32   [6]  in-spans per code"""
     state = state if state is not None else SkipState()
     E = len(out_start)
     labels = labels or list(range(E + 1))
@@ -193,9 +248,8 @@ def solve(engine, in_start, in_end, out_start, out_end, preds, labels=None, stat
     hb, host = marshal(in_start, in_end, s_start, s_end, order, preds, wins, counts, pair, budgets)
     dev = engine.device
     n, nt = len(in_start), len(in_start) * E
-    d = _to_device(host, dev)
-    db = _to_device(hb.arrays, dev)
-    sd = _abi.fill(_abi.TwSkipDesc, d)
+    structs = _descriptors(engine, hb, host)
+    dev_struct, host_struct, sd, _ = structs
     out = dict(assign=torch.empty(nt, dtype=torch.int32, device=dev), mis_rank=torch.empty(n, dtype=torch.int8, device=dev),
                n_cand=torch.empty(n, dtype=torch.int32, device=dev), counters=torch.zeros((1, 4), dtype=torch.int32, device=dev),
                top2_score=torch.empty((n, _abi.TW_K), dtype=torch.float64, device=dev),
@@ -206,12 +260,45 @@ def solve(engine, in_start, in_end, out_start, out_end, preds, labels=None, stat
                    topk_idx=torch.empty(_abi.TW_K * nt, dtype=torch.int32, device=dev),
                    topk_cnt=torch.empty(n, dtype=torch.uint8, device=dev))
     so = _abi.fill(_abi.TwSkipOut, out)
-    dev_struct = batch_struct(hb, lambda name: db[name].data_ptr())
-    host_struct = batch_struct(hb, lambda name: hb.arrays[name].ctypes.data)
     _lib.check(engine.lib.tw_skip_solve(engine.h, C.byref(dev_struct), C.byref(host_struct), C.byref(sd), C.byref(so),
                                         engine.stream), "tw_skip_solve")
+    lk = _assess(engine, structs, n, out["assign"], top2=so) if want_likelihood else None
     engine.status()
     res = to_caller_order({k: v.cpu().numpy() for k, v in out.items()}, order, n, E, want_topk)
     res.update(time_windows=wins, skip_budget=budgets, skip_count=counts, pair_params=pair, large_delay=large_delay,
                sorted_order=order)
+    if want_likelihood:
+        res.update(_likelihood(lk))
     return res
+
+
+def score(engine, in_start, in_end, out_start, out_end, preds, assign, state_snapshot):
+    """The score of ANY assignment of a cache-mode service (the engine's, the ground truth, another
+    predictor's) under the model an earlier `solve` of that service used.  in_start ... preds as given
+    to `solve`; assign [E, n] in the caller's list positions, -1 = ("NA", "NA"), <= -2 = ("Skip", "Skip")
+    (which skip span does not matter); state_snapshot: the dict that `solve` returned (its pair table,
+    budgets, which decide `normalized`, windows and skip counts; with its top2 lists the margin too).
+    Returns host arrays score / code [n] (code TW_ASSESS_* / TW_SKIP_ASSESS_UNDEFINED, score NaN unless
+    code 0), margin [n] when the snapshot has top2 lists, service_score, service_codes [6]."""
+    E, n = len(out_start), len(in_start)
+    assign = np.asarray(assign, np.int32)
+    if assign.shape != (E, n):
+        raise ValueError(f"score: assign must have shape ({E}, {n})")
+    in_start = np.ascontiguousarray(in_start, np.int64)
+    in_end = np.ascontiguousarray(in_end, np.int64)
+    snap = state_snapshot
+    order, s_start, s_end = sort_partitions(out_start, out_end)
+    hb, host = marshal(in_start, in_end, s_start, s_end, order, preds, snap["time_windows"], snap["skip_count"],
+                       snap["pair_params"], snap["skip_budget"])
+    structs = _descriptors(engine, hb, host)
+    top2 = None
+    if "top2_idx" in snap:
+        t2 = _to_device(dict(top2_score=np.ascontiguousarray(snap["top2_score"], np.float64),
+                             top2_idx=to_sorted_order(snap["top2_idx"], order, True).reshape(-1),
+                             top2_cnt=np.ascontiguousarray(snap["top2_cnt"], np.uint8)), engine.device)
+        top2 = _abi.fill(_abi.TwSkipOut, t2)
+    a = _to_device(dict(assign=to_sorted_order(assign, order, False).reshape(-1)), engine.device)["assign"]
+    lk = _assess(engine, structs, n, a, top2)
+    engine.status()
+    res = _likelihood(lk)
+    return dict(score=res.pop("chosen_score"), code=res.pop("chosen_code"), **res)
