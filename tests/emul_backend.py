@@ -79,7 +79,7 @@ class EmulBatch(OracleBatch):
         return res
 
 
-def skip_solve(in_start, in_end, out_start, out_end, preds, wins, counts, pair, budgets, node_limit=4000000):
+def skip_solve(in_start, in_end, out_start, out_end, preds, wins, counts, pair, budgets, node_limit=2000000):
     """k_skip's body (tw_skip_core.cuh) stepped on the CPU, fed through the product's own marshalling
     (traceweaver_b200.skipmode.marshal) with host pointers.  Results in the caller's list order."""
     from traceweaver_b200 import skipmode
