@@ -14,6 +14,10 @@ int two_score_problem(const tw_batch* b, int p, const tw_params* prm, const tw_s
 /* hot loop of one pass, v3:1159-1219 */
 int two_stitch_problem(const tw_batch* b, int p, const tw_params* prm, const uint8_t* cut,
                        const tw_pass_out* out);
+/* a given assignment scored: ScoreAssignmentAsPerInvocationGraph (v1:259-361) after the
+ * feasibility checks of DfsTraverseX (v3:328-347) */
+int two_assess_problem(const tw_batch* b, int p, const tw_params* prm, const int32_t* assign,
+                       double* score, uint8_t* code, double* prob_sum, int32_t* prob_count);
 /* durations of ComputeEpPairDistParams5, v3:721-760 */
 int two_delays(const tw_batch* b, int p, const int32_t* assign, const int64_t* term_sample_off,
                double* delays, int32_t* counts);

@@ -26,13 +26,18 @@ def build(force=False):
     return so
 
 
+def _declare(lib):
+    """The return types of the oracle's entry points (every build of it: this one and tests/oracle_f64.py)."""
+    for name in ("two_params_pass0", "two_score_problem", "two_stitch_problem", "two_assess_problem",
+                 "two_delays", "two_windows_from_cuts", "two_gmm_refit_ex", "two_find_assignments"):
+        getattr(lib, name).restype = C.c_int
+    return lib
+
+
 def lib():
     global _LIB
     if _LIB is None:
-        _LIB = C.CDLL(build())
-        for name in ("two_params_pass0", "two_score_problem", "two_stitch_problem", "two_delays",
-                     "two_windows_from_cuts"):
-            getattr(_LIB, name).restype = C.c_int
+        _LIB = _declare(C.CDLL(build()))
     return _LIB
 
 
@@ -106,6 +111,22 @@ class OracleBatch:
                    "stitch")
         return res
 
+    # -- the likelihood of a given assignment ------------------------------------------------
+    def score_assignments(self, assign, gauss=None, mix=None):
+        """two_assess_problem: score / code per in-span, prob_sum / prob_count per service (scores added in
+        in-span order)."""
+        hb = self.hb
+        n = int(hb.prob_in_off[-1])
+        res = dict(score=np.full(n, np.nan), code=np.zeros(n, np.uint8), prob_sum=np.zeros(hb.n_problems),
+                   prob_count=np.zeros((hb.n_problems, _abi.TW_ASSESS_NCODES), np.int32))
+        prm = self._params_struct(gauss, mix)
+        assign = np.ascontiguousarray(assign, np.int32)
+        for p in range(hb.n_problems):
+            _check(lib().two_assess_problem(C.byref(self.struct), p, C.byref(prm), _ptr(assign),
+                                            _ptr(res["score"]), _ptr(res["code"]), _ptr(res["prob_sum"]),
+                                            _ptr(res["prob_count"])), "score_assignments")
+        return res
+
     def delays(self, assign):
         hb = self.hb
         nt = int(hb.ep_term_off[-1])
@@ -131,7 +152,6 @@ def gmm_refit(term_sample_off, delays, counts, seed_select=10, rng_skip=None):
     """two_gmm_refit_ex: per-term BIC-selected 1-D GMM (restated sklearn, oracle/tw_oracle_gmm.c).
     Returns (mix[n_terms, TW_MIX_REC], n_selected, max_n)."""
     L = lib()
-    L.two_gmm_refit_ex.restype = C.c_int
     nt = len(counts)
     off = np.ascontiguousarray(term_sample_off, np.int64)
     delays = np.ascontiguousarray(delays, np.float64)
@@ -148,7 +168,6 @@ def gmm_refit(term_sample_off, delays, counts, seed_select=10, rng_skip=None):
 def find_assignments(hb: HostBatch, seed_select=10, threads=1, want_topk=True):
     """two_find_assignments: the whole restated path over a batch on `threads` host threads."""
     L = lib()
-    L.two_find_assignments.restype = C.c_int
     n, nt = int(hb.prob_in_off[-1]), int(hb.prob_tuple_off[-1])
     nterm = int(hb.ep_term_off[-1])
     res = dict(assign=np.full(nt, -1, np.int32), mis_rank=np.full(n, -1, np.int8), n_cand=np.zeros(n, np.int32),

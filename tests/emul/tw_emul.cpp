@@ -2,10 +2,12 @@
 //
 // TEST INFRASTRUCTURE ONLY.  The build container has no GPU; this file compiles the very same
 // __host__ __device__ functions the CUDA kernels call (enumerate, score_tuple, topk_offer,
-// bitmaps_intersect, WindowCursor, mwis_solve) with g++ and walks the kernels' thread/warp loops
-// sequentially, so logic errors are caught by `pytest -m "not gpu"` before a GPU call is spent.
-// It is not linked into libtw_b200.so and the package never loads it: the product has no CPU
-// path.  Orchestration mirrors tw_score.cu (k_score) and tw_stitch.cu (k_stitch).
+// bitmaps_intersect, WindowCursor, mwis_solve, assess_in_span, and the skip regime's in tw_skip_core.cuh)
+// with g++ and walks the kernels' thread/warp loops sequentially, so logic errors are caught by
+// `pytest -m "not gpu"` before a GPU call is spent.  It is not linked into libtw_b200.so and the
+// package never loads it: the product has no CPU path.  Orchestration mirrors tw_score.cu (k_score),
+// tw_stitch.cu (k_stitch), tw_assess.cu (k_assess), tw_skip.cu (k_skip) and tw_skip_assess.cu
+// (k_skip_assess).
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -14,20 +16,17 @@
 
 using namespace tw;
 
-// Slots available for term tables (shared memory in the kernels).  Tests set it small to force the
-// lazy per-leaf path and large to force the table path.
-static int g_table_cap = 4096;
-extern "C" void twe_set_table_cap(int cap) { g_table_cap = cap; }
-// In-spans with more than g_light_combos candidate combinations go through the lane-parallel path
-// (32 lanes stride over the combos, partial top-K lists are merged); -1 disables it.
-static long long g_light_combos = -1;
-extern "C" void twe_set_light_combos(long long c) { g_light_combos = c; }
+// Two knobs of twe_score_problem / twe_stitch_problem select the kernels' code paths:
+//   table_cap     term-table slots available per in-span (shared memory in the kernels); in-spans whose
+//                 tables do not fit take the lazy per-leaf path, so 0 forces it.
+//   light_combos  in-spans with more candidate combinations go through the lane-parallel path (32 lanes
+//                 stride over the combos, partial top-K lists are merged); -1 disables it.
 
 // one in-span through the table path: fill -> evaluate every slot -> DFS with look-ups
 template <class Taken>
 static long long enumerate_with_tables(const ProbView& v, const ParamView& pv, int64_t in_s, int64_t in_e,
                                        const OutWin* w, const int* lo, const int* r, int table_size, Taken taken,
-                                       TopK& tk, uint32_t* mark, int W, int* overflow) {
+                                       TopK& tk, uint32_t* mark, int W, int* overflow, long long light_combos) {
   std::vector<double> tbl((size_t)table_size + 1);
   std::vector<uint8_t> sid((size_t)table_size + 1);
   int o_last[TW_MAX_E], lo_abs[TW_MAX_E];
@@ -38,7 +37,7 @@ static long long enumerate_with_tables(const ProbView& v, const ParamView& pv, i
     if (sid[s] != TW_SLOT_INVALID) tbl[s] = term_logpdf(pv, sid[s] & 63, tbl[s]);
   long long leaves = 0;
   const long long P = combo_count(v, r);
-  if (g_light_combos >= 0 && P > g_light_combos && P < (1LL << 40)) {
+  if (light_combos >= 0 && P > light_combos && P < (1LL << 40)) {
     const int L = 32;
     std::vector<TopK> part(L);
     for (int lane = 0; lane < L; ++lane) {
@@ -87,6 +86,8 @@ static long long enumerate_with_tables(const ProbView& v, const ParamView& pv, i
   return leaves;
 }
 
+// the in-span's parameters as the kernels address them: the record of its 100-span batch (pass 0)
+// or the problem's mixture table
 static ParamView param_view(const tw_params* prm, const ProbView& v, int p, int i) {
   ParamView pv;
   pv.mode = prm->mode;
@@ -100,7 +101,7 @@ static ParamView param_view(const tw_params* prm, const ProbView& v, int p, int 
 }
 
 extern "C" int twe_score_problem(const tw_batch* b, int p, const tw_params* prm, const tw_score_out* out,
-                                 int W, int* overflow) {
+                                 int W, int* overflow, int table_cap, long long light_combos) {
   ProbView v;
   int rc = load_view(*b, p, v);
   if (rc) return rc;
@@ -133,9 +134,9 @@ extern "C" int twe_score_problem(const tw_batch* b, int p, const tw_params* prm,
     int r[TW_MAX_E];
     for (int e = 0; e < v.E; ++e) r[e] = range_len(w[e], lo[e], in_e);
     int tsize = term_table_size(v, r);
-    if (prm && tsize <= g_table_cap) {
+    if (prm && tsize <= table_cap) {
       leaves = enumerate_with_tables(v, pv, in_s, in_e, w, lo, r, tsize, [](int, int) { return false; }, tk, mine,
-                                     W, overflow);
+                                     W, overflow, light_combos);
     } else {
       enumerate(v, in_s, in_e, w, lo, [](int, int) { return false; },
                 [&](const int* c, const int64_t* cs, const int64_t* ce) {
@@ -176,7 +177,8 @@ extern "C" int twe_score_problem(const tw_batch* b, int p, const tw_params* prm,
 }
 
 extern "C" int twe_stitch_problem(const tw_batch* b, int p, const tw_params* prm, const uint8_t* cut_all,
-                                  const tw_pass_out* out, long long node_limit) {
+                                  const tw_pass_out* out, long long node_limit, int table_cap,
+                                  long long light_combos) {
   ProbView v;
   int rc = load_view(*b, p, v);
   if (rc) return rc;
@@ -213,9 +215,10 @@ extern "C" int twe_stitch_problem(const tw_batch* b, int p, const tw_params* prm
       for (int e = 0; e < v.E; ++e) r[e] = range_len(w[e], lo[e], in_e);
       int tsize = term_table_size(v, r);
       auto is_taken = [&](int e, int o) { return taken[e][o] != 0; };
-      if (tsize <= g_table_cap) {
+      if (tsize <= table_cap) {
         int ov = 0;
-        leaves = enumerate_with_tables(v, pv, in_s, in_e, w, lo, r, tsize, is_taken, tk, nullptr, 0, &ov);
+        leaves = enumerate_with_tables(v, pv, in_s, in_e, w, lo, r, tsize, is_taken, tk, nullptr, 0, &ov,
+                                       light_combos);
       } else {
         enumerate(v, in_s, in_e, w, lo, is_taken,
                   [&](const int* c, const int64_t* cs, const int64_t* ce) {
@@ -265,6 +268,72 @@ extern "C" int twe_stitch_problem(const tw_batch* b, int p, const tw_params* prm
     out->counters[p * 4 + 3] = 0;
   }
   delete wb;
+  return TW_OK;
+}
+
+static double butterfly32(double* x) {
+  for (int d = 16; d > 0; d >>= 1) {
+    double y[32];
+    for (int l = 0; l < 32; ++l) y[l] = dadd(x[l], x[l ^ d]);
+    for (int l = 0; l < 32; ++l) x[l] = y[l];
+  }
+  return x[0];
+}
+
+// k_assess / k_skip_assess for one problem: assess_one(i, gi) per in-span (thread), the tile partials and
+// their per-service sum in the kernels' order (butterfly over 32 lanes, warps in order, then tile
+// partials strided over 32 lanes and a butterfly).  NC: the code count; `margin` may be NULL.
+template <int NC, class AssessOne>
+static void step_assess(const ProbView& v, int p, AssessOne assess_one, double* score, uint8_t* code,
+                        double* margin, double* prob_sum, int32_t* prob_count) {
+  const int n_tiles = (v.n_in + 127) / 128;
+  std::vector<double> tile_sum((size_t)n_tiles);
+  for (int q = 0; q < NC; ++q) prob_count[(size_t)p * NC + q] = 0;
+  for (int t = 0; t < n_tiles; ++t) {
+    double wsum[4];
+    for (int w = 0; w < 4; ++w) {
+      double lanes[32];
+      for (int l = 0; l < 32; ++l) {
+        const int i = t * 128 + w * 32 + l;
+        lanes[l] = 0.0;
+        if (i >= v.n_in) continue;
+        const int64_t gi = v.in_off + i;
+        const Assessment a = assess_one(i, gi);
+        score[gi] = a.score;
+        code[gi] = (uint8_t)a.code;
+        if (margin) margin[gi] = a.margin;
+        prob_count[(size_t)p * NC + a.code] += 1;
+        if (a.code == TW_ASSESS_SCORED) lanes[l] = a.score;
+      }
+      wsum[w] = butterfly32(lanes);
+    }
+    double s = wsum[0];
+    for (int w = 1; w < 4; ++w) s = dadd(s, wsum[w]);
+    tile_sum[t] = s;
+  }
+  double lanes[32];
+  for (int l = 0; l < 32; ++l) {
+    lanes[l] = 0.0;
+    for (int k = l; k < n_tiles; k += 32) lanes[l] = dadd(lanes[l], tile_sum[k]);
+  }
+  prob_sum[p] = butterfly32(lanes);
+}
+
+// k_assess (tw_assess.cu): assess_in_span per in-span; `top` (a final top-K) may be NULL (no margin)
+extern "C" int twe_assess_problem(const tw_batch* b, int p, const tw_params* prm, const int32_t* assign,
+                                  const tw_score_out* top, double* score, uint8_t* code, double* margin,
+                                  double* prob_sum, int32_t* prob_count) {
+  ProbView v;
+  int rc = load_view(*b, p, v);
+  if (rc) return rc;
+  step_assess<TW_ASSESS_NCODES>(
+      v, p,
+      [&](int i, int64_t gi) {
+        return assess_in_span(v, param_view(prm, v, p, i), i, assign, top ? top->topk_score + gi * TW_K : nullptr,
+                              top ? top->topk_idx + TW_K * (v.tuple_off + (int64_t)i * v.E) : nullptr,
+                              top ? top->topk_cnt[gi] : 0);
+      },
+      score, code, top ? margin : nullptr, prob_sum, prob_count);
   return TW_OK;
 }
 
@@ -420,4 +489,23 @@ extern "C" int twe_skip_solve(const tw_batch* b, const tw_skip_desc* sd, const t
   }
   delete sh;
   return rc;
+}
+
+// k_skip_assess (tw_skip_assess.cu): skip_assess_in_span per in-span; `top2` may be NULL (no margin)
+extern "C" int twe_skip_assess_problem(const tw_batch* b, int p, const tw_skip_desc* sd, const int32_t* assign,
+                                       const tw_skip_out* top2, double* score, uint8_t* code, double* margin,
+                                       double* prob_sum, int32_t* prob_count) {
+  ProbView v;
+  int rc = load_view(*b, p, v);
+  if (rc) return rc;
+  const SkipProb sp = skip_prob(*sd, v, p);
+  step_assess<TW_SKIP_ASSESS_NCODES>(
+      v, p,
+      [&](int i, int64_t gi) {
+        return skip_assess_in_span(v, sp, i, assign, top2 ? top2->top2_score + gi * TW_K : nullptr,
+                                   top2 ? top2->top2_idx + TW_K * (v.tuple_off + (int64_t)i * v.E) : nullptr,
+                                   top2 ? top2->top2_cnt[gi] : 0);
+      },
+      score, code, top2 ? margin : nullptr, prob_sum, prob_count);
+  return TW_OK;
 }

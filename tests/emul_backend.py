@@ -1,5 +1,5 @@
-"""ctypes front end of tests/emul/libtw_emul.so: the engine's device functions (tw_core.cuh)
-compiled for the CPU and stepped sequentially.  Test infrastructure only."""
+"""ctypes front end of tests/emul/libtw_emul.so: the engine's device functions (tw_core.cuh,
+tw_skip_core.cuh) compiled for the CPU and stepped sequentially.  Test infrastructure only."""
 import ctypes as C
 import os
 import subprocess
@@ -21,21 +21,22 @@ def lib():
     return _LIB
 
 
-def set_table_cap(cap):
-    """Term-table slots available per in-span (0 forces the per-leaf path)."""
-    lib().twe_set_table_cap(int(cap))
-
-
-def set_light_combos(c):
-    """In-spans with more candidate combinations than this use the lane-parallel path (-1: never)."""
-    lib().twe_set_light_combos(C.c_longlong(int(c)))
-
-
 class EmulBatch(OracleBatch):
-    """Same interface as OracleBatch, but running the engine's own per-thread code."""
+    """Same interface as OracleBatch, but running the engine's own per-thread code.
+
+    table_cap: term-table slots available per in-span (0 forces the per-leaf path).
+    light_combos: in-spans with more candidate combinations than this use the lane-parallel path (-1: never)."""
 
     W = 2              # bitmap words per (in-span, ep): the narrow kernel's width
     node_limit = 0
+
+    def __init__(self, hb, table_cap=4096, light_combos=-1):
+        super().__init__(hb)
+        self.table_cap = int(table_cap)
+        self.light_combos = int(light_combos)
+
+    def _paths(self):
+        return C.c_int(self.table_cap), C.c_longlong(self.light_combos)
 
     def score(self, gauss=None, mix=None):
         hb = self.hb
@@ -51,11 +52,11 @@ class EmulBatch(OracleBatch):
             ov = C.c_int(0)
             W = self.W
             _check(lib().twe_score_problem(C.byref(self.struct), p, C.byref(prm) if have else None,
-                                           C.byref(out), W, C.byref(ov)), "emul.score")
+                                           C.byref(out), W, C.byref(ov), *self._paths()), "emul.score")
             if ov.value:  # the engine re-runs overflowing tiles with the wide kernel
                 W = 64
                 _check(lib().twe_score_problem(C.byref(self.struct), p, C.byref(prm) if have else None,
-                                               C.byref(out), W, C.byref(ov)), "emul.score")
+                                               C.byref(out), W, C.byref(ov), *self._paths()), "emul.score")
                 assert not ov.value
             self.overflow.append(W)
         return res
@@ -75,19 +76,46 @@ class EmulBatch(OracleBatch):
         cut = np.ascontiguousarray(cut, np.uint8)
         for p in range(hb.n_problems):
             _check(lib().twe_stitch_problem(C.byref(self.struct), p, C.byref(prm), _ptr(cut), C.byref(out),
-                                            C.c_longlong(self.node_limit)), "emul.stitch")
+                                            C.c_longlong(self.node_limit), *self._paths()), "emul.stitch")
+        return res
+
+    def score_assignments(self, assign, gauss=None, mix=None, top=None):
+        """k_assess stepped on the CPU: score / code (/ margin with `top`, a final top-K) per in-span,
+        prob_sum / prob_count per service in the kernels' summation order."""
+        hb = self.hb
+        n, P = int(hb.prob_in_off[-1]), hb.n_problems
+        res = dict(score=np.full(n, -7.0), code=np.full(n, 99, np.uint8), margin=np.full(n, -7.0),
+                   prob_sum=np.zeros(P), prob_count=np.zeros((P, _abi.TW_ASSESS_NCODES), np.int32))
+        prm = self._params_struct(gauss, mix)
+        assign = np.ascontiguousarray(assign, np.int32)
+        tk = None
+        if top is not None:
+            keep = {k: np.ascontiguousarray(top[k]) for k in ("topk_score", "topk_idx", "topk_cnt")}
+            tk = _abi.fill(_abi.TwScoreOut, keep)
+        for p in range(P):
+            _check(lib().twe_assess_problem(C.byref(self.struct), p, C.byref(prm), _ptr(assign),
+                                            C.byref(tk) if tk is not None else None, _ptr(res["score"]),
+                                            _ptr(res["code"]), _ptr(res["margin"]), _ptr(res["prob_sum"]),
+                                            _ptr(res["prob_count"])), "emul.assess")
+        if top is None:
+            del res["margin"]
         return res
 
 
-def skip_solve(in_start, in_end, out_start, out_end, preds, wins, counts, pair, budgets, node_limit=2000000):
-    """k_skip's body (tw_skip_core.cuh) stepped on the CPU, fed through the product's own marshalling
-    (traceweaver_b200.skipmode.marshal) with host pointers.  Results in the caller's list order."""
+def _skip_service(in_start, in_end, out_start, out_end, preds, wins, counts, pair, budgets):
+    """One cache-mode service through the product's own marshalling (traceweaver_b200.skipmode.marshal) with
+    host pointers: the callee lists' sort order, the batch and the skip descriptor's arrays."""
     from traceweaver_b200 import skipmode
-    from traceweaver_b200.batch import batch_struct
-    in_start = np.ascontiguousarray(in_start, np.int64)
-    in_end = np.ascontiguousarray(in_end, np.int64)
     order, s_start, s_end = skipmode.sort_partitions(out_start, out_end)
-    hb, host = skipmode.marshal(in_start, in_end, s_start, s_end, order, preds, wins, counts, pair, budgets)
+    hb, host = skipmode.marshal(np.ascontiguousarray(in_start, np.int64), np.ascontiguousarray(in_end, np.int64),
+                                s_start, s_end, order, preds, wins, counts, pair, budgets)
+    return order, OracleBatch(hb), host
+
+
+def skip_solve(in_start, in_end, out_start, out_end, preds, wins, counts, pair, budgets, node_limit=2000000):
+    """k_skip's body (tw_skip_core.cuh) stepped on the CPU.  Results in the caller's list order."""
+    from traceweaver_b200 import skipmode
+    order, ob, host = _skip_service(in_start, in_end, out_start, out_end, preds, wins, counts, pair, budgets)
     E, n = len(out_start), len(in_start)
     nt = n * E
     out = dict(assign=np.full(nt, -9, np.int32), mis_rank=np.full(n, -9, np.int8), n_cand=np.zeros(n, np.int32),
@@ -97,8 +125,34 @@ def skip_solve(in_start, in_end, out_start, out_end, preds, wins, counts, pair, 
                top2_cnt=np.zeros(n, np.uint8), cut=np.zeros(n, np.uint8))
     sd = _abi.fill(_abi.TwSkipDesc, host)
     so = _abi.fill(_abi.TwSkipOut, out)
-    st = batch_struct(hb, lambda name: _ptr(hb.arrays[name]))
-    L = lib()
-    L.twe_skip_solve.restype = C.c_int
-    _check(L.twe_skip_solve(C.byref(st), C.byref(sd), C.byref(so), C.c_longlong(node_limit)), "emul.skip_solve")
+    _check(lib().twe_skip_solve(C.byref(ob.struct), C.byref(sd), C.byref(so), C.c_longlong(node_limit)),
+           "emul.skip_solve")
     return skipmode.to_caller_order(out, order, n, E)
+
+
+def skip_score(in_start, in_end, out_start, out_end, preds, assign, wins, counts, pair, budgets, top2=None):
+    """k_skip_assess stepped on the CPU over one cache-mode service; assign [E, n] and top2 (top2_score [n, K],
+    top2_idx [n, K, E], top2_cnt [n]) in the caller's list positions.  Returns score / code (/ margin) [n],
+    service_score and service_codes in the kernels' summation order."""
+    from traceweaver_b200 import skipmode
+    order, ob, host = _skip_service(in_start, in_end, out_start, out_end, preds, wins, counts, pair, budgets)
+    n = len(in_start)
+    a = np.ascontiguousarray(skipmode.to_sorted_order(assign, order, False).reshape(-1))
+    res = dict(score=np.full(n, -7.0), code=np.full(n, 99, np.uint8), margin=np.full(n, -7.0), prob_sum=np.zeros(1),
+               prob_count=np.zeros((1, _abi.TW_SKIP_ASSESS_NCODES), np.int32))
+    tk = None
+    if top2 is not None:
+        keep = dict(top2_score=np.ascontiguousarray(top2["top2_score"], np.float64),
+                    top2_idx=np.ascontiguousarray(skipmode.to_sorted_order(top2["top2_idx"], order, True).reshape(-1)),
+                    top2_cnt=np.ascontiguousarray(top2["top2_cnt"], np.uint8))
+        tk = _abi.fill(_abi.TwSkipOut, keep)
+    sd = _abi.fill(_abi.TwSkipDesc, host)
+    _check(lib().twe_skip_assess_problem(C.byref(ob.struct), 0, C.byref(sd), _ptr(a),
+                                         C.byref(tk) if tk is not None else None, _ptr(res["score"]),
+                                         _ptr(res["code"]), _ptr(res["margin"]), _ptr(res["prob_sum"]),
+                                         _ptr(res["prob_count"])), "emul.skip_assess")
+    out = dict(score=res["score"], code=res["code"], service_score=float(res["prob_sum"][0]),
+               service_codes=res["prob_count"][0])
+    if top2 is not None:
+        out["margin"] = res["margin"]
+    return out

@@ -94,10 +94,7 @@ def _load_frontend():
     spec = importlib.util.spec_from_file_location("tw_oracle_f64_frontend", os.path.join(ORACLE, "tw_oracle.py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
-    lib = C.CDLL(build())
-    for name in ("two_params_pass0", "two_score_problem", "two_stitch_problem", "two_delays", "two_windows_from_cuts"):
-        getattr(lib, name).restype = C.c_int
-    mod._LIB = lib
+    mod._LIB = mod._declare(C.CDLL(build()))
     return mod
 
 

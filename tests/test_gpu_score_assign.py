@@ -6,7 +6,7 @@ import pytest
 
 from float_times_util import SOLVABLE, compress
 from golden_util import Golden, golden_files
-from assess_backends import oracle_score
+from oracle.tw_oracle import OracleBatch
 from test_score_assign import host_margin, rank_assign
 
 pytestmark = pytest.mark.gpu
@@ -157,14 +157,14 @@ def test_golden_tuples_and_truth(engine, golden_batch):
         for r in range(K):
             a = _rank_assign_batch(hb, idx, cnt, r)
             got = eng.score_assignments(prm, _dev(a, eng))
-            orc = oracle_score(hb, a, **kw)
+            orc = OracleBatch(hb).score_assignments(a, **kw)
             live = cnt > r
             g, ref = _np(got["score"])[live], want[live, r]
             assert np.array_equal(_np(got["code"]), orc["code"])
             assert np.array_equal(np.isnan(g), np.isnan(ref))
             assert np.max(np.abs(g - ref), where=~np.isnan(ref), initial=0.0) < TOL
         lk = eng.score_assignments(prm, _dev(truth, eng))
-        orc = oracle_score(hb, truth, **kw)
+        orc = OracleBatch(hb).score_assignments(truth, **kw)
         code = _np(lk["code"])
         assert np.array_equal(code, orc["code"])
         assert np.array_equal(_np(lk["prob_count"]), orc["prob_count"])
@@ -179,7 +179,7 @@ def test_golden_tuples_and_truth(engine, golden_batch):
 def _check_solve_outputs(out, hb, probs=None):
     """chosen_code 1 exactly where assign has -1; chosen_score = the oracle's score of the chosen tuple
     under the returned mixtures; margin as defined; service sums against a host sum."""
-    orc = oracle_score(hb, out["assign"], mix=out["mixtures"])
+    orc = OracleBatch(hb).score_assignments(out["assign"], mix=out["mixtures"])
     code, score = out["chosen_code"], out["chosen_score"]
     for p in range(hb.n_problems):
         i0, i1 = int(hb.prob_in_off[p]), int(hb.prob_in_off[p + 1])
@@ -213,7 +213,7 @@ def test_solve_likelihood_outputs(solver, golden_batch, batches):
 def test_solver_scores_the_truth(solver, golden_batch):
     hb, probs, gauss, mix, truth = golden_batch
     res = solver.score(hb, truth, mix)
-    orc = oracle_score(hb, truth, mix=mix)
+    orc = OracleBatch(hb).score_assignments(truth, mix=mix)
     assert np.array_equal(res["code"], orc["code"])
     assert np.array_equal(res["service_codes"], orc["prob_count"])
     ok = res["code"] == 0
@@ -283,6 +283,7 @@ def test_integral_float_binds_bit_identical(solver, golden_batch):
 def test_compressed_fixtures_match_the_float_oracle(engine, goldens):
     """Compression divides start times and keeps durations, so the uncompressed truth is mostly infeasible
     there (code 4, as in the float oracle); the engine's own final tuples are scored under its own model."""
+    import oracle_f64
     from traceweaver_b200.batch import build_batch
     from traceweaver_b200.predictor import solve_bound
     sel = [g for g in goldens if g.path.split("/")[-1][:-4] in SOLVABLE[3]]
@@ -300,7 +301,7 @@ def test_compressed_fixtures_match_the_float_oracle(engine, goldens):
     for prm, kw in ((res["params_pass1"], dict(mix=mix)), (p0, dict(gauss=gauss))):
         for a in (truth, _np(res["assign"]), rank0):
             lk = eng.score_assignments(prm, _dev(a, eng))
-            orc = oracle_score(hb, a, **kw, float_times=True)
+            orc = oracle_f64.OracleBatch(hb).score_assignments(a, **kw)
             code, s = _np(lk["code"]), _np(lk["score"])
             assert np.array_equal(code, orc["code"])
             assert np.array_equal(np.isnan(s), np.isnan(orc["score"]))

@@ -3,12 +3,13 @@ running the reference's own executor.py + TraceWeaverV3 in the build container
 (tests/golden/make_goldens.py).  The same checks run on "emul": the engine's device functions
 (traceweaver_b200/csrc/tw_core.cuh) compiled for the CPU and stepped thread by thread
 (tests/emul/), because the build container has no GPU.  CPU only."""
+from functools import partial
+
 import numpy as np
 import pytest
 
 from golden_util import Golden, golden_files
 from oracle import tw_oracle
-import emul_backend
 from emul_backend import EmulBatch
 from traceweaver_b200 import _abi
 from traceweaver_b200.batch import build_batch
@@ -22,41 +23,10 @@ def test_goldens_present():
     assert len(FILES) >= 10
 
 
-class EmulLazy(EmulBatch):
-    """Same device functions with the term tables disabled (per-leaf evaluation path)."""
-
-    def score(self, *a, **k):
-        emul_backend.set_table_cap(0)
-        try:
-            return super().score(*a, **k)
-        finally:
-            emul_backend.set_table_cap(4096)
-
-    def stitch(self, *a, **k):
-        emul_backend.set_table_cap(0)
-        try:
-            return super().stitch(*a, **k)
-        finally:
-            emul_backend.set_table_cap(4096)
-
-
-class EmulCombos(EmulBatch):
-    """Every in-span through the lane-parallel combination path + partial top-K merge."""
-
-    def score(self, *a, **k):
-        emul_backend.set_light_combos(0)
-        try:
-            return super().score(*a, **k)
-        finally:
-            emul_backend.set_light_combos(-1)
-
-    def stitch(self, *a, **k):
-        emul_backend.set_light_combos(0)
-        try:
-            return super().stitch(*a, **k)
-        finally:
-            emul_backend.set_light_combos(-1)
-
+# Same device functions with the term tables disabled (per-leaf evaluation path)
+EmulLazy = partial(EmulBatch, table_cap=0)
+# Every in-span through the lane-parallel combination path + partial top-K merge
+EmulCombos = partial(EmulBatch, light_combos=0)
 
 BACKENDS = {"oracle": tw_oracle.OracleBatch, "emul": EmulBatch, "emul-lazy": EmulLazy, "emul-combos": EmulCombos}
 

@@ -4,8 +4,9 @@ per-in-span device function (assess_in_span, tw_core.cuh) stepped on the CPU aga
 import numpy as np
 import pytest
 
-from assess_backends import emul_score, oracle_score
+from emul_backend import EmulBatch
 from golden_util import Golden, golden_files
+from oracle.tw_oracle import OracleBatch
 from traceweaver_b200 import _abi
 from traceweaver_b200.batch import Problem, build_batch
 
@@ -62,7 +63,7 @@ def test_oracle_scores_golden_tuples(case, pass_id, which):
         live = cnt > r
         if not live.any():
             break
-        res = oracle_score(hb, rank_assign(idx, cnt, r), **_params(g, prob, pass_id))
+        res = OracleBatch(hb).score_assignments(rank_assign(idx, cnt, r), **_params(g, prob, pass_id))
         assert np.all(res["code"][live] == _abi.TW_ASSESS_SCORED)
         assert np.all(res["code"][~live] == _abi.TW_ASSESS_NA)
         got, ref = res["score"][live], want[live, r]
@@ -73,7 +74,7 @@ def test_oracle_scores_golden_tuples(case, pass_id, which):
 
 def test_oracle_scores_the_truth(case):
     g, prob, hb = case
-    res = oracle_score(hb, g.z["truth"].astype(np.int32).reshape(-1), mix=g.mix_table(prob))
+    res = OracleBatch(hb).score_assignments(g.z["truth"].astype(np.int32).reshape(-1), mix=g.mix_table(prob))
     code, score = res["code"], res["score"]
     assert np.all(code < _abi.TW_ASSESS_NCODES)
     assert np.all(np.isfinite(score[code == 0])) and np.all(np.isnan(score[code != 0]))
@@ -81,7 +82,7 @@ def test_oracle_scores_the_truth(case):
     assert res["prob_sum"][0] == pytest.approx(score[code == 0].sum(), rel=1e-12, abs=1e-12)
     # the reference's own assignment of the last pass is feasible everywhere it assigned
     a = g.z["assign"].astype(np.int32)
-    res = oracle_score(hb, a.reshape(-1), mix=g.mix_table(prob))
+    res = OracleBatch(hb).score_assignments(a.reshape(-1), mix=g.mix_table(prob))
     assert np.array_equal(res["code"] == _abi.TW_ASSESS_NA, (a < 0).any(axis=0))
     assert np.all(res["code"][(a >= 0).all(axis=0)] == _abi.TW_ASSESS_SCORED)
 
@@ -95,8 +96,8 @@ def test_device_function_equals_oracle(case):
                topk_cnt=g.z["topk2_cnt"][1].astype(np.uint8))
     for a in (g.z["assign"], g.z["truth"], g.z["topk2_idx"][1][:, 1, :].T):
         a = np.ascontiguousarray(a, np.int32).reshape(-1)
-        want = oracle_score(hb, a, mix=mix)
-        got = emul_score(hb, a, mix=mix, top=top)
+        want = OracleBatch(hb).score_assignments(a, mix=mix)
+        got = EmulBatch(hb).score_assignments(a, mix=mix, top=top)
         assert np.array_equal(got["code"], want["code"])
         assert np.array_equal(got["prob_count"], want["prob_count"])
         ok = want["code"] == 0
@@ -108,7 +109,7 @@ def test_device_function_equals_oracle(case):
     # pass-0 parameters: the record of the in-span's 100-span batch
     gauss = g.gauss_table(prob)
     a = rank_assign(g.z["topk2_idx"][0], g.z["topk2_cnt"][0], 0)
-    got = emul_score(hb, a, gauss=gauss)
+    got = EmulBatch(hb).score_assignments(a, gauss=gauss)
     live = g.z["topk2_cnt"][0] > 0
     ref = g.z["topk2_score"][0][live, 0]
     assert np.array_equal(np.isnan(got["score"][live]), np.isnan(ref))
@@ -136,16 +137,16 @@ def test_crafted_codes():
     nterm = int(hb.ep_term_off[-1])
     mix = np.zeros((nterm, _abi.TW_MIX_REC))
     mix[:, 1:4] = (20.0, 5.0, np.log(5.0))             # k = 0: a Gaussian record
-    res = oracle_score(hb, assign.reshape(-1), mix=mix)
+    res = OracleBatch(hb).score_assignments(assign.reshape(-1), mix=mix)
     assert res["code"].tolist() == want
     assert np.isfinite(res["score"][0]) and np.all(np.isnan(res["score"][1:]))
     assert res["prob_count"][0].tolist() == [1, 1, 1, 1, 1]
     assert res["prob_sum"][0] == res["score"][0]
-    got = emul_score(hb, assign.reshape(-1), mix=mix)
+    got = EmulBatch(hb).score_assignments(assign.reshape(-1), mix=mix)
     assert got["code"].tolist() == want
     assert abs(got["score"][0] - res["score"][0]) < TOL
     # the lowest code wins: an NA and an out-of-range index in one tuple is NA
     a = assign.copy()
     a[1, 1] = 9
-    assert oracle_score(hb, a.reshape(-1), mix=mix)["code"][1] == _abi.TW_ASSESS_NA
-    assert emul_score(hb, a.reshape(-1), mix=mix)["code"][1] == _abi.TW_ASSESS_NA
+    assert OracleBatch(hb).score_assignments(a.reshape(-1), mix=mix)["code"][1] == _abi.TW_ASSESS_NA
+    assert EmulBatch(hb).score_assignments(a.reshape(-1), mix=mix)["code"][1] == _abi.TW_ASSESS_NA

@@ -5,8 +5,8 @@ the goldens and the oracle, and crafted tuples for every feasibility code."""
 import numpy as np
 import pytest
 
-from assess.skip_emul_assess import emul_skip_score
 from assess.skip_oracle_assess import assess, assess_service, scorer
+from emul_backend import skip_score
 from golden_util import Golden
 from oracle import tw_oracle_skip as osk
 from test_skip_mode import FILES, IDS
@@ -68,8 +68,8 @@ def host_margin(score, code, assign, top2_score, top2_idx, top2_cnt):
 
 
 def _emul(prob, md, assign, top2=None):
-    return emul_skip_score(prob.in_start, prob.in_end, prob.out_start, prob.out_end, prob.preds, assign, md["wins"],
-                           md["counts"], md["tab"], md["budgets"], top2=top2)
+    return skip_score(prob.in_start, prob.in_end, prob.out_start, prob.out_end, prob.preds, assign, md["wins"],
+                      md["counts"], md["tab"], md["budgets"], top2=top2)
 
 
 def _oracle(prob, md, assign):
