@@ -20,7 +20,9 @@ using namespace tw;
 //   table_cap     term-table slots available per in-span (shared memory in the kernels); in-spans whose
 //                 tables do not fit take the lazy per-leaf path, so 0 forces it.
 //   light_combos  in-spans with more candidate combinations go through the lane-parallel path (32 lanes
-//                 stride over the combos, partial top-K lists are merged); -1 disables it.
+//                 stride over the combos, partial top-K lists are merged); -1 disables it.  As in step 1
+//                 of warp_topk_search (tw_score.cu) and its copy in the stitch, an equal score or a NaN
+//                 among the six best sends the in-span back to the sequential heap replay.
 
 // one in-span through the table path: fill -> evaluate every slot -> DFS with look-ups
 template <class Taken>
@@ -40,6 +42,7 @@ static long long enumerate_with_tables(const ProbView& v, const ParamView& pv, i
   if (light_combos >= 0 && P > light_combos && P < (1LL << 40)) {
     const int L = 32;
     std::vector<TopK> part(L);
+    bool tie = false;
     for (int lane = 0; lane < L; ++lane) {
       part[lane].n = 0;
       enumerate_combos(v, w, lo, r, o_last, sid.data(), lane, L, P,
@@ -51,25 +54,39 @@ static long long enumerate_with_tables(const ProbView& v, const ParamView& pv, i
                              if (bit >= 32 * W) { *overflow = 1; continue; }
                              mark[e * W + (bit >> 5)] |= 1u << (bit & 31);
                            }
-                         topk_offer_sorted(v, part[lane], table_score(v, r, lo_abs, tbl.data(), c, ce), c);
+                         const double sc = table_score(v, r, lo_abs, tbl.data(), c, ce);
+                         for (int k = 0; k < part[lane].n; ++k) tie = tie || part[lane].score[k] == sc;
+                         tie = tie || sc != sc;
+                         topk_offer_sorted(v, part[lane], sc, c);
                        });
     }
+    // K + 1 rounds of "best head over the lanes": a maximum held by two lanes, or equal to the previous
+    // round's, is a tie among the six best
     int head[32] = {0};
-    for (int k = 0; k < TW_K; ++k) {      // K rounds of "best head over the lanes"
-      int best = -1;
-      for (int lane = 0; lane < L; ++lane) {
-        if (head[lane] >= part[lane].n) continue;
-        if (best < 0 || cand_ahead(v, part[lane].score[head[lane]], part[lane].idx[head[lane]],
-                                   part[best].score[head[best]], part[best].idx[head[best]]))
-          best = lane;
+    double prev = 0.0;
+    for (int round = 0; round <= TW_K; ++round) {
+      double mx = -INFINITY;
+      for (int lane = 0; lane < L; ++lane)
+        if (head[lane] < part[lane].n && part[lane].score[head[lane]] > mx) mx = part[lane].score[head[lane]];
+      if (!(mx > -INFINITY)) break;
+      int best = -1, holders = 0;
+      for (int lane = 0; lane < L; ++lane)
+        if (head[lane] < part[lane].n && part[lane].score[head[lane]] == mx) {
+          if (best < 0) best = lane;
+          ++holders;
+        }
+      if (holders > 1 || (round > 0 && mx == prev)) tie = true;
+      prev = mx;
+      if (round < TW_K) {
+        tk.score[tk.n] = mx;
+        for (int e = 0; e < v.E; ++e) tk.idx[tk.n][e] = part[best].idx[head[best]][e];
+        ++tk.n;
       }
-      if (best < 0) break;
-      tk.score[tk.n] = part[best].score[head[best]];
-      for (int e = 0; e < v.E; ++e) tk.idx[tk.n][e] = part[best].idx[head[best]][e];
-      ++tk.n;
       ++head[best];
     }
-    return leaves;
+    if (!tie) return leaves;
+    tk.clear();                            // the owner redoes the in-span alone (step 2)
+    leaves = 0;
   }
   enumerate(v, in_s, in_e, w, lo,
             [&](int e, int o) { return sid[o_last[e] + (o - lo_abs[e])] == TW_SLOT_INVALID; },

@@ -11,6 +11,9 @@ re-sorted afterwards, so they arrive partly out of order.  `extra` adds spans th
 `run_oracle` runs `oracle/tw_oracle_skip.solve_skip` with its branches counted (sys.monitoring on the
 oracle's own code objects, nothing in the oracle changes), so the tests can say which branches the
 generated inputs reach.
+
+`dag_problem` builds two-pass services (no cache hits) on the DAGs of DAG_SHAPES with the same laws,
+for the tests of services with five to eight callees (tests/test_dag_shapes.py).
 """
 import inspect
 import sys
@@ -48,7 +51,7 @@ class SkipService:
         return len(self.in_start)
 
 
-def _dag_trace_times(spec, n, load, seed, quantum):
+def dag_trace_times(spec, n, load, seed, quantum):
     """make_block's laws on a DAG: [n] in-span times, per-callee [n] span times of trace i."""
     rng = np.random.default_rng(seed)
     ia = np.maximum(np.rint(rng.exponential(spec["ia100"] * 100.0 / load, size=n)), 1).astype(np.int64)
@@ -69,7 +72,7 @@ def _dag_trace_times(spec, n, load, seed, quantum):
 def _traces(shape, n, load, seed, quantum):
     """(in_s, in_e, starts [E][n], ends [E][n], preds) with trace i's call of callee e at [e][i]."""
     if shape == "dag8":
-        in_s, in_e, st, en = _dag_trace_times(DAG8, n, load, seed, quantum)
+        in_s, in_e, st, en = dag_trace_times(DAG8, n, load, seed, quantum)
         o = np.lexsort((in_e, in_s))
         return in_s[o], in_e[o], [s[o] for s in st], [x[o] for x in en], DAG8["preds"]
     blk = synth.make_block(shape, 1, n_in=n, load=load, seed=seed, quantum_us=quantum)
@@ -77,6 +80,46 @@ def _traces(shape, n, load, seed, quantum):
     st = [blk.out_start[e][0][tr[e]] for e in range(len(blk.out_start))]
     en = [blk.out_end[e][0][tr[e]] for e in range(len(blk.out_start))]
     return blk.in_start[0].copy(), blk.in_end[0].copy(), st, en, blk.preds
+
+
+# Two-pass services on DAGs no synth.SHAPES entry has (predecessor lists in in_edges order, which is the
+# order the score sums a callee's edge terms in): name -> (preds, number of score terms)
+_EPS, _TAIL = DAG8["eps"][0], DAG8["tail"]
+DAG_SHAPES = {
+    "dag8": (DAG8["preds"], 17),
+    # K4,4: four parallel roots, four sinks after all of them (in scrambled in_edges order): the most
+    # terms a service of eight callees can have (4 roots + 16 edges + 8 lasts)
+    "k44": ([[], [], [], [], [3, 1, 0, 2], [0, 1, 2, 3], [2, 3, 1, 0], [1, 0, 3, 2]], 28),
+    "k33": ([[], [], [], [2, 0, 1], [1, 2, 0], [0, 1, 2]], 18),
+    "mix7": ([[], [], [0], [0, 1], [3], [2, 4], [5, 1]], 17),
+    "dag5": ([[], [0], [0], [2, 1], [1]], 11),
+    # every callee after the one and the two before it: each transitive edge e-2 -> e is non-primary
+    "chain8": ([[]] + [[e - 1] + ([e - 2] if e >= 2 else []) for e in range(1, 8)], 16),
+    "diamond": ([[], [0], [0], [2, 1, 0]], 9),
+}
+
+
+def dag_problem(shape, n=260, ia_us=12_000.0, seed=0, quantum=1):
+    """One two-pass service of DAG_SHAPES[shape] (batch.Problem) and its truth [E, n] (position of trace
+    i's call in callee e's list): `n` in-spans with a mean inter-arrival of `ia_us`, timestamps rounded
+    down to `quantum` us, in-spans and callee lists in (start, end) order like synth.make_block's."""
+    from traceweaver_b200.batch import Problem
+    preds = DAG_SHAPES[shape][0]
+    E = len(preds)
+    spec = dict(preds=preds, eps=[_EPS] * E, tail=_TAIL, ia100=ia_us)
+    in_s, in_e, st, en = dag_trace_times(spec, n, 100.0, seed, quantum)
+    o = np.lexsort((in_e, in_s))
+    in_s, in_e, st, en = in_s[o], in_e[o], [s[o] for s in st], [x[o] for x in en]
+    out_s, out_e = [], []
+    truth = np.empty((E, n), np.int32)
+    for e in range(E):
+        od = np.lexsort((en[e], st[e]))
+        truth[e, od] = np.arange(n)
+        out_s.append(np.ascontiguousarray(st[e][od]))
+        out_e.append(np.ascontiguousarray(en[e][od]))
+    prob = Problem(in_start=np.ascontiguousarray(in_s), in_end=np.ascontiguousarray(in_e), out_start=out_s,
+                   out_end=out_e, preds=[list(p) for p in preds], name=f"{shape}-n{n}-ia{ia_us:g}-s{seed}-q{quantum}")
+    return prob, truth
 
 
 def make_service(shape, n=120, load=60.0, seed=0, cached=(), rate=0.0, quantum=1, extra=(), shift=0):

@@ -28,9 +28,18 @@ def _run(nw, E, cnt, score, idx):
 
 @pytest.mark.parametrize("seed", range(300))
 def test_exhaustive_search_equals_branch_and_bound(seed):
-    rng = np.random.default_rng(seed)
+    _check(np.random.default_rng(seed), 1, 4, seed)
+
+
+@pytest.mark.parametrize("seed", range(300, 900))
+def test_exhaustive_search_equals_branch_and_bound_five_to_eight_callees(seed):
+    """Tuples of 5..8 spans: the per-position conflict test runs over every callee, not the first four."""
+    _check(np.random.default_rng(seed), 5, 8, seed)
+
+
+def _check(rng, e_min, e_max, seed):
     nw = int(rng.integers(2, 7))
-    E = int(rng.integers(1, 5))
+    E = int(rng.integers(e_min, e_max + 1))
     n_spans = int(rng.integers(2, 9))                      # few distinct spans: many conflicts
     cnt = rng.integers(0, 6, nw)
     score = np.full((nw, 5), np.nan)
