@@ -1,13 +1,23 @@
 // tw_emul.cpp — CPU stepping of the engine's per-thread device functions (tw_core.cuh).
 //
-// TEST INFRASTRUCTURE ONLY.  The build container has no GPU; this file compiles the very same
-// __host__ __device__ functions the CUDA kernels call (enumerate, score_tuple, topk_offer,
-// bitmaps_intersect, WindowCursor, mwis_solve, assess_in_span, and the skip regime's in tw_skip_core.cuh)
-// with g++ and walks the kernels' thread/warp loops sequentially, so logic errors are caught by
-// `pytest -m "not gpu"` before a GPU call is spent.  It is not linked into libtw_b200.so and the
-// package never loads it: the product has no CPU path.  Orchestration mirrors tw_score.cu (k_score),
-// tw_stitch.cu (k_stitch), tw_assess.cu (k_assess), tw_skip.cu (k_skip) and tw_skip_assess.cu
-// (k_skip_assess).
+// TEST INFRASTRUCTURE ONLY, for machines without a GPU: logic errors are caught by `pytest -m "not gpu"`
+// before a GPU run is spent.  It is not linked into libtw_b200.so and the package never loads it: the
+// product has no CPU path.
+//
+// The device functions themselves, compiled here with g++ from the headers the kernels include:
+// load_view, param_view, term_logpdf / score_tuple, enumerate, the term tables (term_table_* ,
+// table_score, enumerate_combos), the top-K list (topk_offer, topk_offer_sorted, topk_finish,
+// store_topk_row), bitmaps_intersect, WindowCursor, window_adjacency, mwis_solve, assignment_solve,
+// the small-window search (small_component, small_strides, small_leaf, SmallBest::offer / merge,
+// small_decode), assess_in_span, and the whole skip regime of tw_skip_core.cuh.
+//
+// Orchestration written for the CPU, mirroring tw_score.cu (k_score), tw_stitch.cu (k_stitch),
+// tw_assess.cu (k_assess), tw_skip.cu (k_skip) and tw_skip_assess.cu (k_skip_assess) but not shared
+// with them: the loops over threads, lanes and butterfly steps; the prev-index scan and the cut flags
+// of twe_score_problem; the K + 1 head-merge rounds of the heavy-in-span path in enumerate_with_tables
+// (ballots and shuffles in the kernels); the conflict masks of twe_small_window (__match_any_sync in
+// the kernel); the taken bitmap as a byte array.  The kernels' tiers that only choose where a list
+// comes from (run / adopt in k_stitch, the work-balanced k_score3) have no counterpart here.
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -103,20 +113,6 @@ static long long enumerate_with_tables(const ProbView& v, const ParamView& pv, i
   return leaves;
 }
 
-// the in-span's parameters as the kernels address them: the record of its 100-span batch (pass 0)
-// or the problem's mixture table
-static ParamView param_view(const tw_params* prm, const ProbView& v, int p, int i) {
-  ParamView pv;
-  pv.mode = prm->mode;
-  pv.gauss = nullptr;
-  pv.mix = nullptr;
-  if (prm->mode == TW_PARAMS_GAUSS_BATCHED)
-    pv.gauss = prm->gauss + (prm->prob_gauss_off[p] + (int64_t)(i / TW_PARAM_BATCH) * v.n_terms) * TW_GAUSS_REC;
-  else
-    pv.mix = prm->mix + (int64_t)v.term0 * TW_MIX_REC;
-  return pv;
-}
-
 extern "C" int twe_score_problem(const tw_batch* b, int p, const tw_params* prm, const tw_score_out* out,
                                  int W, int* overflow, int table_cap, long long light_combos) {
   ProbView v;
@@ -146,7 +142,7 @@ extern "C" int twe_score_problem(const tw_batch* b, int p, const tw_params* prm,
     long long leaves = 0;
     uint32_t* mine = &used[(size_t)i * TW_MAX_E * W];
     ParamView pv;
-    if (prm) pv = param_view(prm, v, p, i);
+    if (prm) pv = param_view(*prm, v, p, i / TW_PARAM_BATCH, nullptr);
     int64_t in_s = v.is[i], in_e = v.ie[i];
     int r[TW_MAX_E];
     for (int e = 0; e < v.E; ++e) r[e] = range_len(w[e], lo[e], in_e);
@@ -168,14 +164,9 @@ extern "C" int twe_score_problem(const tw_batch* b, int p, const tw_params* prm,
     }
     topk_finish(v, tk);
     out->n_feasible[v.in_off + i] = (int32_t)leaves;
-    if (prm && out->topk_score) {
-      out->topk_cnt[v.in_off + i] = (uint8_t)tk.n;
-      for (int k = 0; k < TW_K; ++k) {
-        out->topk_score[(v.in_off + i) * TW_K + k] = k < tk.n ? tk.score[k] : NAN;
-        for (int e = 0; e < v.E; ++e)
-          out->topk_idx[TW_K * (v.tuple_off + (int64_t)i * v.E) + k * v.E + e] = k < tk.n ? tk.idx[k][e] : -1;
-      }
-    }
+    if (prm && out->topk_score)
+      store_topk_row(tk, v.E, out->topk_score + (v.in_off + i) * TW_K,
+                     out->topk_idx + TW_K * (v.tuple_off + (int64_t)i * v.E), out->topk_cnt + v.in_off + i);
   }
   for (int i = 0; i < n; ++i) {
     uint8_t cut = 0;
@@ -226,7 +217,7 @@ extern "C" int twe_stitch_problem(const tw_batch* b, int p, const tw_params* prm
       if (l == 0) for (int e = 0; e < v.E; ++e) cursor[e] = lo[e];
       TopK tk; tk.clear();
       long long leaves = 0;
-      ParamView pv = param_view(prm, v, p, i);
+      const ParamView pv = param_view(*prm, v, p, i / TW_PARAM_BATCH, nullptr);
       int64_t in_s = v.is[i], in_e = v.ie[i];
       int r[TW_MAX_E];
       for (int e = 0; e < v.E; ++e) r[e] = range_len(w[e], lo[e], in_e);
@@ -250,14 +241,9 @@ extern "C" int twe_stitch_problem(const tw_batch* b, int p, const tw_params* prm
         wb->score[l][k] = tk.score[k];
         for (int e = 0; e < v.E; ++e) wb->idx[l][k][e] = tk.idx[k][e];
       }
-      if (out->topk_score) {
-        out->topk_cnt[v.in_off + i] = (uint8_t)tk.n;
-        for (int k = 0; k < TW_K; ++k) {
-          out->topk_score[(v.in_off + i) * TW_K + k] = k < tk.n ? tk.score[k] : NAN;
-          for (int e = 0; e < v.E; ++e)
-            out->topk_idx[TW_K * (v.tuple_off + (int64_t)i * v.E) + k * v.E + e] = k < tk.n ? tk.idx[k][e] : -1;
-        }
-      }
+      if (out->topk_score)
+        store_topk_row(tk, v.E, out->topk_score + (v.in_off + i) * TW_K,
+                       out->topk_idx + TW_K * (v.tuple_off + (int64_t)i * v.E), out->topk_cnt + v.in_off + i);
     }
     if (closes) {
       for (int l = 0; l < nw; ++l) wb->adj[l] = window_adjacency(*wb, v.E, nw, l);
@@ -346,7 +332,7 @@ extern "C" int twe_assess_problem(const tw_batch* b, int p, const tw_params* prm
   step_assess<TW_ASSESS_NCODES>(
       v, p,
       [&](int i, int64_t gi) {
-        return assess_in_span(v, param_view(prm, v, p, i), i, assign, top ? top->topk_score + gi * TW_K : nullptr,
+        return assess_in_span(v, param_view(*prm, v, p, i / TW_PARAM_BATCH, nullptr), i, assign, top ? top->topk_score + gi * TW_K : nullptr,
                               top ? top->topk_idx + TW_K * (v.tuple_off + (int64_t)i * v.E) : nullptr,
                               top ? top->topk_cnt[gi] : 0);
       },
@@ -387,97 +373,59 @@ extern "C" long long twe_mwis_window(int nw, int E, const int* cnt, const double
   return nodes;
 }
 
-// The warp-parallel solver of tw_stitch.cu (stitch_small_window) restated for one thread: candidate
-// (k, r) = "lane" 5k + r, conflict masks per candidate, components of the in-span conflict graph,
-// exhaustive mixed-radix enumeration (lowest in-span most significant, digit cnt = unassigned),
-// the lowest combination index among the totals tied with the largest (TW_MWIS_TIE_TOL).  Returns 0 when the kernel would fall back
-// to the sequential solver (E == 1 component of >= 3 in-spans, or more than `space_cap` leaves).
+// stitch_small_window (tw_stitch.cu) stepped lane by lane: the component search, the leaves, each lane's
+// running best and the merge of the lanes are the kernel's own functions (tw_core.cuh, small_component
+// .. SmallBest).  Written out here: what the kernel gets from warp collectives — the validity ballot,
+// the conflict masks of __match_any_sync, the atomicOr into the in-span adjacency — and the loops over
+// the 32 lanes and the five butterfly steps.  Returns 0 when the kernel would fall back to the
+// sequential solver (E == 1 component of >= 3 in-spans, or more than `space_cap` leaves).
 extern "C" int twe_small_window(int nw, int E, const int* cnt_in, const double* score, const int* idx,
                                 int* chosen, int space_cap) {
-  const int KW = 6;
-  if (nw > KW) return 0;
-  uint32_t conf[32] = {0};
+  if (nw > kSmallWindow) return 0;
+  uint32_t cconf[32] = {0};
   double cw[32] = {0};
-  auto valid = [&](int c) { int k = c / TW_K, r = c % TW_K; return k < nw && r < cnt_in[k]; };
-  for (int a = 0; a < 32; ++a) {
-    if (!valid(a)) continue;
-    cw[a] = TW_WEIGHT_OFFSET + score[a];
-    for (int b = 0; b < 32; ++b) {
-      if (!valid(b) || a / TW_K == b / TW_K) continue;
+  int cnt[kSmallWindow];
+  uint32_t adj[kSmallWindow] = {0};
+  for (int a = 0; a < kSmallWindow; ++a) cnt[a] = a < nw ? cnt_in[a] : 0;
+  auto valid = [&](int lane) { return lane / TW_K < nw && lane % TW_K < cnt_in[lane / TW_K]; };
+  for (int lane = 0; lane < 32; ++lane) {
+    if (!valid(lane)) continue;
+    cw[lane] = TW_WEIGHT_OFFSET + score[lane];
+    for (int o = 0; o < 32; ++o) {
+      if (!valid(o) || o / TW_K == lane / TW_K) continue;
       for (int e = 0; e < E; ++e)
-        if (idx[a * E + e] == idx[b * E + e]) conf[a] |= 1u << b;
+        if (idx[lane * E + e] == idx[o * E + e]) cconf[lane] |= 1u << o;
     }
+    for (int a = 0; a < kSmallWindow; ++a)
+      if ((cconf[lane] >> (TW_K * a)) & 0x1fu) adj[lane / TW_K] |= 1u << a;
   }
-  uint32_t adj[KW] = {0};
-  for (int a = 0; a < 32; ++a)
-    for (int q = 0; q < KW; ++q)
-      if ((conf[a] >> (TW_K * q)) & 0x1fu) adj[a / TW_K] |= 1u << q;
   for (int k = 0; k < nw; ++k) chosen[k] = -1;
   uint32_t todo = (1u << nw) - 1u;
   while (todo) {
-    int seed = 0;
-    while (!(todo >> seed & 1u)) ++seed;
-    uint32_t comp = 1u << seed, frontier = comp;
-    while (frontier) {
-      int q = 0;
-      while (!(frontier >> q & 1u)) ++q;
-      frontier &= frontier - 1u;
-      uint32_t nb = adj[q] & ~comp;
-      comp |= nb;
-      frontier |= nb;
-    }
+    const int seed = lowest_bit(todo);
+    const uint32_t comp = small_component(adj, seed);
     todo &= ~comp;
-    int m = 0;
-    for (int a = 0; a < KW; ++a) m += (comp >> a) & 1u;
+    const int m = __builtin_popcount(comp);
     if (m == 1) {
-      if (cnt_in[seed] > 0 && cw[TW_K * seed] > 0.0) chosen[seed] = 0;
+      if (cnt[seed] > 0 && cw[TW_K * seed] > 0.0) chosen[seed] = 0;
       continue;
     }
     if (E == 1 && m >= 3) return 0;
-    int stride[KW], space = 1;
-    for (int a = KW - 1; a >= 0; --a) {
-      stride[a] = space;
-      if ((comp >> a) & 1u) space *= (a < nw ? cnt_in[a] : 0) + 1;
-    }
+    int stride[kSmallWindow];
+    const int space = small_strides(comp, cnt, stride);
     if (space > space_cap) return 0;
-    // two passes like the kernel: the maximum total, then the lowest leaf index tied with it
-    auto leaf_total = [&](int id, bool& ok) {
-      int rem = id;
-      uint32_t sel = 0;
-      double tot = 0.0;
-      ok = true;
-      for (int a = 0; a < KW; ++a) {
-        if (!((comp >> a) & 1u)) continue;
-        int d = rem / stride[a];
-        rem -= d * stride[a];
-        if (d < cnt_in[a]) {
-          int c = TW_K * a + d;
-          if (!(cw[c] > 0.0) || (conf[c] & sel)) ok = false;
-          sel |= 1u << c;
-          tot = tot + cw[c];
-        }
+    SmallBest best[32];
+    for (int lane = 0; lane < 32; ++lane)
+      for (int leaf = lane; leaf < space; leaf += 32) {
+        double tot;
+        if (small_leaf(comp, cnt, stride, cw, cconf, leaf, &tot)) best[lane].offer(tot, leaf);
       }
-      return tot;
-    };
-    double best_w = -1.0;
-    for (int id = 0; id < space; ++id) {
-      bool ok;
-      const double tot = leaf_total(id, ok);
-      if (ok && tot > best_w) best_w = tot;
+    for (int d = 16; d > 0; d >>= 1) {
+      SmallBest before[32];
+      for (int lane = 0; lane < 32; ++lane) before[lane] = best[lane];
+      for (int lane = 0; lane < 32; ++lane) best[lane].merge(before[lane ^ d]);
     }
-    int best_idx = 0x7fffffff;
-    for (int id = 0; id < space && best_idx == 0x7fffffff; ++id) {
-      bool ok;
-      const double tot = leaf_total(id, ok);
-      if (ok && tot >= best_w - TW_MWIS_TIE_TOL) best_idx = id;
-    }
-    int rem = best_idx;
-    for (int a = 0; a < KW; ++a) {
-      if (!((comp >> a) & 1u)) continue;
-      int d = rem / stride[a];
-      rem -= d * stride[a];
-      chosen[a] = d < cnt_in[a] ? d : -1;
-    }
+    small_decode(comp, cnt, stride, best[0].idx, [&](int a, int rank) { chosen[a] = rank; });
   }
   return 1;
 }

@@ -2,7 +2,9 @@
 (tw_stitch.cu: stitch_small_window) instead of the sequential branch and bound.  Its rule —
 largest total, then the first leaf in depth-first order — must pick exactly what mwis_solve picks,
 ties included.  Both are stepped on the CPU here (tests/emul): mwis_solve is the device function
-itself, the exhaustive search a one-thread restatement of the kernel's lanes."""
+itself, and so are the exhaustive search's leaves, each lane's running best and the butterfly merge of
+the 32 lanes (tw_core.cuh); only the conflict masks the kernel takes from __match_any_sync are written
+out for the CPU."""
 import ctypes as C
 
 import numpy as np

@@ -21,13 +21,7 @@ k_assess(tw_batch b, tw_params prm, const int32_t* __restrict__ assign, tw_score
   int code = -1;
   double sc = 0.0;
   if (i < v.n_in) {
-    ParamView pv;
-    pv.mode = prm.mode;
-    pv.gauss = prm.mode == TW_PARAMS_GAUSS_BATCHED
-                   ? prm.gauss + (prm.prob_gauss_off[p] + (int64_t)(i / TW_PARAM_BATCH) * v.n_terms) * TW_GAUSS_REC
-                   : nullptr;
-    pv.mix = prm.mode == TW_PARAMS_MIXTURE ? prm.mix + (int64_t)v.term0 * TW_MIX_REC : nullptr;
-    pv.etab = etab;
+    const ParamView pv = param_view(prm, v, p, i / TW_PARAM_BATCH, etab);
     const int64_t gi = v.in_off + i;
     const Assessment a =
         assess_in_span(v, pv, i, assign, with_top ? top.topk_score + gi * TW_K : nullptr,

@@ -43,6 +43,25 @@ TW_HD double dsub(double a, double b) { volatile double r = a - b; return r; }
 TW_HD double ddiv(double a, double b) { volatile double r = a / b; return r; }
 #endif
 
+// the quiet NaN that fills the unused ranks of every top-K output row
+TW_HD double tw_nan() {
+  const uint64_t bits = 0x7ff8000000000000ULL;
+  double d;
+  memcpy(&d, &bits, sizeof d);
+  return d;
+}
+
+// index of the lowest set bit (m != 0)
+TW_HD int lowest_bit(uint32_t m) {
+#if defined(__CUDA_ARCH__)
+  return __ffs(m) - 1;
+#else
+  int k = 0;
+  while (!(m >> k & 1u)) ++k;
+  return k;
+#endif
+}
+
 // ---------------------------------------------------------------------------------------------
 // Likelihood terms: GetEpPairCost, V1:117-139.
 // ---------------------------------------------------------------------------------------------
@@ -133,6 +152,26 @@ struct ParamView {
   const double* mix;
   const double* etab = nullptr;   // device: shared-memory copy of c_exp2_64 -> branch-free mixture path
 };
+
+// The view of an in-span in 100-span batch `batch`, counted from the batch whose Gaussian records
+// start at `gauss0` (the service's first batch in global memory, or the first batch a tile staged).
+// A caller that staged one table of the mode in use passes it as both bases.
+TW_HD ParamView param_view(int mode, const double* gauss0, const double* mix, int batch, int n_terms,
+                           const double* etab) {
+  ParamView pv;
+  pv.mode = mode;
+  pv.gauss = mode == TW_PARAMS_GAUSS_BATCHED ? gauss0 + (int64_t)batch * n_terms * TW_GAUSS_REC : nullptr;
+  pv.mix = mix;
+  pv.etab = etab;
+  return pv;
+}
+// ... of service p, from the batch's parameter arrays (in-span i is in batch i / TW_PARAM_BATCH)
+TW_HD ParamView param_view(const tw_params& prm, const ProbView& v, int p, int batch, const double* etab) {
+  return param_view(prm.mode,
+                    prm.mode == TW_PARAMS_GAUSS_BATCHED ? prm.gauss + prm.prob_gauss_off[p] * TW_GAUSS_REC : nullptr,
+                    prm.mode == TW_PARAMS_MIXTURE ? prm.mix + (int64_t)v.term0 * TW_MIX_REC : nullptr, batch,
+                    v.n_terms, etab);
+}
 
 #ifdef __CUDACC__
 // exp(d) for d in [-40, 0], branch free (callers discard the value for d < -40): d = (64 q + j) ln2/64
@@ -341,6 +380,16 @@ struct TopK {
     for (int k = 0; k <= TW_K; ++k) heap[k] = (uint8_t)k;
   }
 };
+
+// A finished list (topk_finish) as an in-span's row of a top-K output: score_row[TW_K] and
+// idx_row[TW_K][E] hold the tk.n filled ranks, then NaN / -1.
+TW_HD void store_topk_row(const TopK& tk, int E, double* score_row, int32_t* idx_row, uint8_t* cnt) {
+  *cnt = (uint8_t)tk.n;
+  for (int k = 0; k < TW_K; ++k) {
+    score_row[k] = k < tk.n ? tk.score[k] : tw_nan();
+    for (int e = 0; e < E; ++e) idx_row[k * E + e] = k < tk.n ? tk.idx[k][e] : -1;
+  }
+}
 
 // a < b in the reference's (score, stack) order: tuple comparison takes the score first; on equal
 // scores the stacks are compared element by element, the first position holding two different Span
@@ -1232,6 +1281,110 @@ TW_HD_NOINLINE inline long long mwis_solve(WB& wb, int E, int nw, long long node
   }
   return nodes;
 }
+
+// ---------------------------------------------------------------------------------------------
+// Windows of <= kSmallWindow in-spans: exhaustive search by 32 lanes (stitch_small_window,
+// tw_stitch.cu).  Candidate (in-span k, rank r) is "lane" 5k + r: cw[] holds its weight (0 when the
+// slot is empty), cconf[] the mask of the candidates of other in-spans it shares an out span with.
+// Every connected component is enumerated: leaf index = mixed-radix number over the component's
+// in-spans, lowest in-span most significant, digit r = "take rank r", digit cnt = "leave unassigned"
+// — exactly the order in which mwis_solve's depth-first search reaches the leaves, so "largest
+// total, first in that order" is the solution the sequential branch and bound returns (its bound
+// only discards subtrees that cannot strictly improve).  Totals are summed in level order like cur[]
+// there.  Below is what one lane does on its own; the per-in-span arrays are indexed by unrolled
+// constants only, so they stay in registers.
+// ---------------------------------------------------------------------------------------------
+constexpr int kSmallWindow = 6;
+constexpr int kSmallSpace = 4096;   // a component with more leaves goes to the sequential solver
+
+// connected component of in-span `seed`; bit a of adj[k] <=> in-spans k and a conflict
+TW_HD uint32_t small_component(const uint32_t (&adj)[kSmallWindow], int seed) {
+  uint32_t comp = 1u << seed, frontier = comp;
+  while (frontier) {
+    const int q = lowest_bit(frontier);
+    frontier &= frontier - 1u;
+    uint32_t nb = 0u;
+#pragma unroll
+    for (int a = 0; a < kSmallWindow; ++a) nb = a == q ? adj[a] : nb;
+    nb &= ~comp;
+    comp |= nb;
+    frontier |= nb;
+  }
+  return comp;
+}
+
+// radix (cnt + 1) for the in-spans of the component, 1 for the others; stride of in-span a = product
+// of the radices after it.  Returns the number of leaves.
+TW_HD int small_strides(uint32_t comp, const int (&cnt)[kSmallWindow], int (&stride)[kSmallWindow]) {
+  int space = 1;
+#pragma unroll
+  for (int a = kSmallWindow - 1; a >= 0; --a) {
+    stride[a] = space;
+    if ((comp >> a) & 1u) space *= cnt[a] + 1;
+  }
+  return space;
+}
+
+// leaf `idx` of the component: false when it takes a candidate of weight <= 0 or two that conflict
+TW_HD bool small_leaf(uint32_t comp, const int (&cnt)[kSmallWindow], const int (&stride)[kSmallWindow],
+                      const double* cw, const uint32_t* cconf, int idx, double* total) {
+  int rem = idx;
+  uint32_t sel = 0u;
+  double tot = 0.0;
+  bool ok = true;
+#pragma unroll
+  for (int a = 0; a < kSmallWindow; ++a) {
+    if ((comp >> a) & 1u) {
+      const int d = rem / stride[a];
+      rem -= d * stride[a];
+      if (d < cnt[a]) {
+        const int c = TW_K * a + d;
+        const double wgt = cw[c];
+        if (!(wgt > 0.0) || (cconf[c] & sel)) ok = false;
+        sel |= 1u << c;
+        tot = tot + wgt;
+      }
+    }
+  }
+  *total = tot;
+  return ok;
+}
+
+// put(a, rank) for every in-span a of the component: its digit of leaf `idx` (-1 = unassigned)
+template <class Put>
+TW_HD void small_decode(uint32_t comp, const int (&cnt)[kSmallWindow], const int (&stride)[kSmallWindow], int idx,
+                        Put put) {
+  int rem = idx;
+#pragma unroll
+  for (int a = 0; a < kSmallWindow; ++a) {
+    if ((comp >> a) & 1u) {
+      const int d = rem / stride[a];
+      rem -= d * stride[a];
+      put(a, d < cnt[a] ? d : -1);
+    }
+  }
+}
+
+// (largest total seen, first leaf tied with it).  Totals are either tied (equal up to rounding, far
+// below TW_MWIS_TIE_TOL) or apart by more than the tolerance, so "first leaf tied with the maximum"
+// is what the sequential search returns, whatever the order in which totals were rounded.
+struct SmallBest {
+  double w = -1.0;
+  int idx = 0x7fffffff;
+  // the lane's next feasible leaf; a lane offers its leaves in ascending order
+  TW_HD void offer(double total, int leaf) {
+    const bool better = total > w + TW_MWIS_TIE_TOL;              // a better group; else the same group keeps its first leaf
+    idx = better ? leaf : idx;
+    w = better || total > w ? total : w;
+  }
+  // one step of the xor butterfly over the lanes (selects, like offer: the kernel's merge stays branch free)
+  TW_HD void merge(const SmallBest& o) {
+    const bool better = o.w > w + TW_MWIS_TIE_TOL;
+    const bool tied = !better && !(w > o.w + TW_MWIS_TIE_TOL);   // tied groups: the earlier leaf, the larger total
+    idx = better || (tied && o.idx < idx) ? o.idx : idx;
+    w = better || (tied && o.w > w) ? o.w : w;
+  }
+};
 
 // ---------------------------------------------------------------------------------------------
 // Windows from cut flags: CreateWindows2's loop, V3:1056-1076, as a cursor the stitch kernel

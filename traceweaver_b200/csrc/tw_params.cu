@@ -148,7 +148,7 @@ __device__ __forceinline__ double tstd_dev(const double* x, int n) {
   double d[TW_PARAM_NBATCHES];
   for (int i = 0; i < n; ++i) { double t = dsub(x[i], mean); d[i] = dmul(t, t); }
   double var = ddiv(np_sum10(d, n), (double)n);
-  if (n - 1 <= 0) return __longlong_as_double(0x7ff8000000000000LL);
+  if (n - 1 <= 0) return tw_nan();
   var = dmul(var, ddiv((double)n, (double)(n - 1)));
   return sqrt(var);
 }

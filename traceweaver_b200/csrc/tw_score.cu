@@ -378,14 +378,9 @@ __device__ __forceinline__ void score_tile(const tw_batch& b, const tw_params& p
   auto write_out = [&](const TopK& tk, int leaves) {
     int64_t gi = v.in_off + i;
     out.n_feasible[gi] = leaves;
-    if (do_score && out.topk_score) {
-      out.topk_cnt[gi] = (uint8_t)tk.n;
-      int32_t* ix = out.topk_idx + TW_K * (v.tuple_off + (int64_t)i * E);
-      for (int k = 0; k < TW_K; ++k) {
-        out.topk_score[gi * TW_K + k] = k < tk.n ? tk.score[k] : __longlong_as_double(0x7ff8000000000000LL);
-        for (int e = 0; e < E; ++e) ix[k * E + e] = k < tk.n ? tk.idx[k][e] : -1;
-      }
-    }
+    if (do_score && out.topk_score)
+      store_topk_row(tk, E, out.topk_score + gi * TW_K, out.topk_idx + TW_K * (v.tuple_off + (int64_t)i * E),
+                     out.topk_cnt + gi);
   };
   // windows-only launches and the carry-in helper only mark (no likelihoods)
   if ((worker || helper) && !do_score) {
@@ -399,12 +394,7 @@ __device__ __forceinline__ void score_tile(const tw_batch& b, const tw_params& p
   }
   // ---- scoring; every scored in-span is a worker, whose windows are the tile's staged ones
   auto params = [&](int bq) {   // the staged tables: mixtures, or the Gaussians of batch batch0 + bq
-    ParamView pv;
-    pv.mode = prm.mode;
-    pv.gauss = sm.prm + bq * v.n_terms * TW_GAUSS_REC;
-    pv.mix = sm.prm;
-    pv.etab = sm.etab;
-    return pv;
+    return param_view(prm.mode, sm.prm, sm.prm, bq, v.n_terms, sm.etab);
   };
   warp_topk_search<kTblCap, kRedoCoopCombos>(v, sm.win, params, batch0, sm.tbl, sm.sid, tid, i, in_s, in_e, lo, do_score,
                                              [](int, int) { return false; }, mark, write_out);

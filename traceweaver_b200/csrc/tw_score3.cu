@@ -180,12 +180,7 @@ __device__ __forceinline__ double key_to_score3(unsigned long long k) {
 // one likelihood value on a rare path (kept out of line so the hot loops stay small)
 __device__ __noinline__ double term_logpdf_cold(int mode, const double* rec_base, int n_terms, int brel, int t,
                                                 const double* etab, double dt) {
-  ParamView pv;
-  pv.mode = mode;
-  pv.gauss = rec_base + brel * n_terms * TW_GAUSS_REC;
-  pv.mix = rec_base;
-  pv.etab = etab;
-  return term_logpdf(pv, t, dt);
+  return term_logpdf(param_view(mode, rec_base, rec_base, brel, n_terms, etab), t, dt);
 }
 
 // coalesced copy of `nwords` 32-bit words from shared to global memory by one warp: 128-bit stores
@@ -729,7 +724,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
   if (has_params) {
     const int kc = (tk0 != 0) + (tk1 != 0) + (tk2 != 0) + (tk3 != 0) + (tk4 != 0);
     if (worker) out.topk_cnt[g0 + lane] = (uint8_t)kc;
-    const double nan = __longlong_as_double(0x7ff8000000000000LL);
+    const double nan = tw_nan();
     double* sd = ws.tbl;
     sd[lane * TW_K + 0] = tk0 ? key_to_score3(tk0) : nan;
     sd[lane * TW_K + 1] = tk1 ? key_to_score3(tk1) : nan;

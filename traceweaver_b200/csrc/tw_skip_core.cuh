@@ -5,26 +5,11 @@
 
 namespace tw {
 
-TW_HD double tw_nan() {
-  const uint64_t bits = 0x7ff8000000000000ULL;
-  double d;
-  memcpy(&d, &bits, sizeof d);
-  return d;
-}
-
-
-
 constexpr int kSkipCand = 96;                    // candidates of one ep inside one in-span
 constexpr int kSkipTouched = 384;                // bitmap words a candidate set may touch before it is cleared wholesale
 constexpr double kSqrt2Pi = 2.5066282746310002;  // scipy _norm_pdf_C = sqrt(2 pi)
 constexpr double kLogSqrt2Pi = 0.91893853320467274178;   // _norm_pdf_logC
 constexpr double kFixedScale = 4398046511104.0;  // 2^42: weights in [2^10, 2^14) are integers at this scale
-
-TW_HD int lowest_bit(uint32_t m) {
-  int k = 0;
-  while (!(m >> k & 1u)) ++k;
-  return k;
-}
 
 struct SkipProb {
   int n_win;
@@ -534,24 +519,15 @@ TW_HD_NOINLINE inline int skip_solve_problem(const tw_batch& b, int p, const tw_
       sh.wb.score[nw][r] = sh.tk.score[r];
       for (int e = 0; e < E; ++e) sh.wb.idx[nw][r][e] = sh.tk.idx[r][e];
     }
-    if (want_topk) {
-      out.pass.topk_cnt[gi] = (uint8_t)sh.tk.n;
-      for (int r = 0; r < TW_K; ++r) {
-        out.pass.topk_score[gi * TW_K + r] = r < sh.tk.n ? sh.tk.score[r] : tw_nan();
-        for (int e = 0; e < E; ++e)
-          out.pass.topk_idx[TW_K * (v.tuple_off + (int64_t)i * E) + r * E + e] = r < sh.tk.n ? sh.tk.idx[r][e] : -1;
-      }
-    }
+    if (want_topk)
+      store_topk_row(sh.tk, E, out.pass.topk_score + gi * TW_K,
+                     out.pass.topk_idx + TW_K * (v.tuple_off + (int64_t)i * E), out.pass.topk_cnt + gi);
     ++nw;
     // top_k_2 on the undeleted, sorted lists (V3:1185) -> all_topk_assignments
     skip_topk(v, sp, sh, i, w, false, taken, taken_off, err_flag);
     if (status != TW_OK) return status;
-    out.top2_cnt[gi] = (uint8_t)sh.tk.n;
-    for (int r = 0; r < TW_K; ++r) {
-      out.top2_score[gi * TW_K + r] = r < sh.tk.n ? sh.tk.score[r] : tw_nan();
-      for (int e = 0; e < E; ++e)
-        out.top2_idx[TW_K * (v.tuple_off + (int64_t)i * E) + r * E + e] = r < sh.tk.n ? sh.tk.idx[r][e] : -1;
-    }
+    store_topk_row(sh.tk, E, out.top2_score + gi * TW_K, out.top2_idx + TW_K * (v.tuple_off + (int64_t)i * E),
+                   out.top2_cnt + gi);
     if (!wc.ends_at(i, n, cut)) continue;
     // ---- window end: MWIS, assignment, deletion
     const long long nodes = skip_mwis(sh, E, nw, node_limit);

@@ -59,18 +59,12 @@ struct StitchSlab {
   }
 };
 
-// Exact MWIS of a window of <= 6 in-spans by the whole warp.  Candidate (in-span k, rank r) lives in
-// lane 5k + r; its conflicts with the other candidates come from one __match_any_sync per tuple
-// position (AssignmentIntersect, V3:1276-1281).  Every connected component of the in-span conflict
-// graph is then enumerated exhaustively: combination index = mixed-radix number over the
-// component's in-spans, lowest in-span most significant, digit r = "take rank r", digit cnt =
-// "leave unassigned" — exactly the order in which mwis_solve's depth-first search reaches the
-// leaves, so "largest total, first in that order" is the solution the sequential branch and bound
-// returns (its bound only discards subtrees that cannot strictly improve).  Totals are summed in
-// level order like cur[] there.  Returns false (nothing decided) when a component needs the
-// sequential solver: E == 1 with >= 3 in-spans (Hungarian path) or more than kSmallSpace leaves.
-constexpr int kSmallWindow = 6;
-constexpr int kSmallSpace = 4096;
+// Exact MWIS of a window of <= kSmallWindow in-spans by the whole warp (the search and its tie rule:
+// tw_core.cuh, small_component .. SmallBest).  Here is what the warp does together: the conflicts of
+// candidate lane 5k + r with the other candidates come from one __match_any_sync per tuple position
+// (AssignmentIntersect, V3:1276-1281), the lanes take the leaves lane, lane + 32, ... of a component
+// and an xor butterfly merges their bests.  Returns false (nothing decided) when a component needs
+// the sequential solver: E == 1 with >= 3 in-spans (Hungarian path) or more than kSmallSpace leaves.
 __device__ __forceinline__ bool stitch_small_window(StitchWarpSmem& sm, PackedWindowBuf& wb, int E, int nw, int lane,
                                                     long long* nodes_out) {
   const unsigned kAll = 0xffffffffu;
@@ -99,18 +93,8 @@ __device__ __forceinline__ bool stitch_small_window(StitchWarpSmem& sm, PackedWi
   long long nodes = 0;
   uint32_t todo = (1u << nw) - 1u;
   while (todo) {
-    const int seed = __ffs(todo) - 1;
-    uint32_t comp = 1u << seed, frontier = comp;
-    while (frontier) {
-      const int q = __ffs(frontier) - 1;
-      frontier &= frontier - 1u;
-      uint32_t nb = 0u;
-#pragma unroll
-      for (int a = 0; a < kSmallWindow; ++a) nb = a == q ? adj[a] : nb;
-      nb &= ~comp;
-      comp |= nb;
-      frontier |= nb;
-    }
+    const int seed = lowest_bit(todo);
+    const uint32_t comp = small_component(adj, seed);
     todo &= ~comp;
     const int m = __popc(comp);
     if (m == 1) {   // isolated in-span: its best candidate, if the weight is positive
@@ -119,67 +103,24 @@ __device__ __forceinline__ bool stitch_small_window(StitchWarpSmem& sm, PackedWi
       continue;
     }
     if (E == 1 && m >= 3) return false;
-    // radix (cnt + 1) for the in-spans of the component, 1 for the others; stride of in-span a =
-    // product of the radices after it
     int stride[kSmallWindow];
-    int space = 1;
-#pragma unroll
-    for (int a = kSmallWindow - 1; a >= 0; --a) {
-      stride[a] = space;
-      if ((comp >> a) & 1u) space *= cnt[a] + 1;
-    }
+    const int space = small_strides(comp, cnt, stride);
     if (space > kSmallSpace) return false;
-    // One pass: every lane keeps (largest total seen, first leaf tied with it) over its leaves, the
-    // warp then merges the pairs.  Totals are either tied (equal up to rounding, far below
-    // TW_MWIS_TIE_TOL) or apart by more than the tolerance, so "first leaf tied with the maximum"
-    // is what the sequential search returns, whatever the order in which totals were rounded.
-    double best_w = -1.0;
-    int best_idx = 0x7fffffff;
+    SmallBest best;
     for (int idx = lane; idx < space; idx += 32) {
-      int rem = idx;
-      uint32_t sel = 0u;
-      double tot = 0.0;
-      bool ok = true;
-#pragma unroll
-      for (int a = 0; a < kSmallWindow; ++a) {
-        if ((comp >> a) & 1u) {
-          const int d = rem / stride[a];
-          rem -= d * stride[a];
-          if (d < cnt[a]) {
-            const int c = TW_K * a + d;
-            const double wgt = sm.cw[c];
-            if (!(wgt > 0.0) || (sm.cconf[c] & sel)) ok = false;
-            sel |= 1u << c;
-            tot = tot + wgt;
-          }
-        }
-      }
-      if (ok) {
-        if (tot > best_w + TW_MWIS_TIE_TOL) { best_w = tot; best_idx = idx; }   // a better group
-        else if (tot > best_w) best_w = tot;                                    // same group: keep the first leaf
-      }
+      double tot;
+      if (small_leaf(comp, cnt, stride, sm.cw, sm.cconf, idx, &tot)) best.offer(tot, idx);
     }
 #pragma unroll
     for (int d = 16; d > 0; d >>= 1) {
-      const double ow = __shfl_xor_sync(kAll, best_w, d);
-      const int oi = __shfl_xor_sync(kAll, best_idx, d);
-      if (ow > best_w + TW_MWIS_TIE_TOL) { best_w = ow; best_idx = oi; }
-      else if (!(best_w > ow + TW_MWIS_TIE_TOL)) {      // tied groups: the earlier leaf, the larger total
-        best_idx = oi < best_idx ? oi : best_idx;
-        best_w = ow > best_w ? ow : best_w;
-      }
+      SmallBest other;
+      other.w = __shfl_xor_sync(kAll, best.w, d);
+      other.idx = __shfl_xor_sync(kAll, best.idx, d);
+      best.merge(other);
     }
-    {
-      int rem = best_idx;
-#pragma unroll
-      for (int a = 0; a < kSmallWindow; ++a) {
-        if ((comp >> a) & 1u) {
-          const int d = rem / stride[a];
-          rem -= d * stride[a];
-          if (lane == 0) wb.chosen[a] = d < cnt[a] ? d : -1;
-        }
-      }
-    }
+    small_decode(comp, cnt, stride, best.idx, [&](int a, int rank) {
+      if (lane == 0) wb.chosen[a] = rank;
+    });
     nodes += space;
   }
   *nodes_out = nodes;
@@ -370,14 +311,9 @@ __device__ __noinline__ void stitch_search_lanes(const ProbView& v, PackedWindow
       wb.score[lane][k] = tk.score[k];
       for (int e = 0; e < E; ++e) wb.at(lane, k, e) = tk.idx[k][e];
     }
-    if (out.topk_score) {
-      out.topk_cnt[gi] = (uint8_t)tk.n;
-      int32_t* ix = out.topk_idx + TW_K * (v.tuple_off + (int64_t)i * E);
-      for (int k = 0; k < TW_K; ++k) {
-        out.topk_score[gi * TW_K + k] = k < tk.n ? tk.score[k] : __longlong_as_double(0x7ff8000000000000LL);
-        for (int e = 0; e < E; ++e) ix[k * E + e] = k < tk.n ? tk.idx[k][e] : -1;
-      }
-    }
+    if (out.topk_score)
+      store_topk_row(tk, E, out.topk_score + gi * TW_K, out.topk_idx + TW_K * (v.tuple_off + (int64_t)i * E),
+                     out.topk_cnt + gi);
   };
   bool pending = active;
   // ---- heavy in-spans (thousands of candidate combinations), one at a time by the WHOLE warp:
@@ -405,14 +341,9 @@ __device__ __noinline__ void stitch_search_lanes(const ProbView& v, PackedWindow
       __syncwarp();
       for (int sl = lane; sl < tsz; sl += 32) {
         const uint8_t id = tb.sid[sl];
-        if (id != TW_SLOT_INVALID) {
-          ParamView pv;
-          pv.mode = prm.mode;
-          pv.gauss = gauss_base ? gauss_base + (int64_t)(batch0 + (id >> 6)) * v.n_terms * TW_GAUSS_REC : nullptr;
-          pv.mix = mix_base;
-          pv.etab = etab;
-          tb.tbl[sl] = term_logpdf(pv, id & 63, tb.tbl[sl]);
-        }
+        if (id != TW_SLOT_INVALID)
+          tb.tbl[sl] = term_logpdf(param_view(prm.mode, gauss_base, mix_base, batch0 + (id >> 6), v.n_terms, etab),
+                                   id & 63, tb.tbl[sl]);
       }
       __syncwarp();
       TopK part;
@@ -483,11 +414,7 @@ __device__ __noinline__ void stitch_search_lanes(const ProbView& v, PackedWindow
       term_table_fill(v, in_s, in_e, w, lo, r, o_last, brel, is_taken, tb.tbl + offset, tb.sid + offset);
     }
     if (lazy) {   // tables larger than the warp's StitchTables: evaluate per leaf
-      ParamView pv;
-      pv.mode = prm.mode;
-      pv.gauss = gauss_base ? gauss_base + (int64_t)(i / TW_PARAM_BATCH) * v.n_terms * TW_GAUSS_REC : nullptr;
-      pv.mix = mix_base;
-      pv.etab = etab;
+      const ParamView pv = param_view(prm.mode, gauss_base, mix_base, i / TW_PARAM_BATCH, v.n_terms, etab);
       TopK tk;
       tk.clear();
       int leaves = 0;
@@ -503,14 +430,9 @@ __device__ __noinline__ void stitch_search_lanes(const ProbView& v, PackedWindow
     __syncwarp();
     for (int s = lane; s < total; s += 32) {     // GetEpPairCost for every slot, all lanes busy
       const uint8_t id = tb.sid[s];
-      if (id != TW_SLOT_INVALID) {
-        ParamView pv;
-        pv.mode = prm.mode;
-        pv.gauss = gauss_base ? gauss_base + (int64_t)(batch0 + (id >> 6)) * v.n_terms * TW_GAUSS_REC : nullptr;
-        pv.mix = mix_base;
-        pv.etab = etab;
-        tb.tbl[s] = term_logpdf(pv, id & 63, tb.tbl[s]);
-      }
+      if (id != TW_SLOT_INVALID)
+        tb.tbl[s] = term_logpdf(param_view(prm.mode, gauss_base, mix_base, batch0 + (id >> 6), v.n_terms, etab),
+                                id & 63, tb.tbl[s]);
     }
     __syncwarp();
     if (in_round) {
@@ -626,7 +548,7 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
     out.mis_rank[v.in_off + i] = -1;
     for (int e = 0; e < E; ++e) out.assign[v.tuple_off + (int64_t)e * n + i] = -1;
   }
-
+  // the bases param_view(mode, ...) takes in the search tier, as param_view(prm, ...) computes them
   const double* gauss_base = prm.mode == TW_PARAMS_GAUSS_BATCHED
                                  ? prm.gauss + prm.prob_gauss_off[p] * TW_GAUSS_REC : nullptr;
   const double* mix_base = prm.mode == TW_PARAMS_MIXTURE ? prm.mix + (int64_t)v.term0 * TW_MIX_REC : nullptr;
