@@ -110,8 +110,11 @@ struct tw_engine {
   DevBuf<int32_t> unit_hi;
   DevBuf<int> unit_count;
   int max_units = 0;
+  int unit_min = kStitchUnitMin;     // shortest unit of the bound batch (bind)
   StitchLayout stitch_layout{};      // per-warp shared memory of k_stitch for the bound batch
-  DevBuf<StitchTables> stitch_tables;   // search tables, one per stitch warp
+  int stitch_blocks = 0;             // persistent grid of k_stitch (bind; tw_debug_stitch_grid)
+  int stitch_blocks_max = 0;         // the grid the bind sized stitch_tables for
+  DevBuf<StitchTables> stitch_tables;   // search tables, one per warp of the grid
   DevBuf<int32_t> long_seg;          // lists longer than kSortSmemCap (sorted in global memory)
   int n_long = 0;
   DevBuf<int64_t> long_scratch;
@@ -330,18 +333,8 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
   CU(up(eng->ep_prob.p, ep_prob));
   CU(cudaStreamSynchronize(s));   // staging vectors go out of scope
 
-  // unit list of the stitch kernel: at most n / kStitchUnitMin + 1 units per service
-  {
-    int64_t mu = 0;
-    for (int p = 0; p < P; ++p) mu += (h->prob_in_off[p + 1] - h->prob_in_off[p]) / kStitchUnitMin + 1;
-    if (mu > 0x7fffffff) return fail(TW_ERR_RANGE_LIMIT, "bind: too many stitch units");
-    eng->max_units = (int)mu;
-    CU(eng->unit_prob.reserve((size_t)mu));
-    CU(eng->unit_lo.reserve((size_t)mu));
-    CU(eng->unit_hi.reserve((size_t)mu));
-    CU(eng->unit_count.reserve(1));
-  }
   // shared-memory slab of a stitch warp: sized for the batch's largest E and largest taken bitmap
+  int stitch_resident = 0;   // blocks of k_stitch the device holds at once with this slab
   {
     int e_max = 1, tk_max = 0;
     for (int p = 0; p < P; ++p) {
@@ -352,7 +345,28 @@ int tw_engine_bind(tw_engine* eng, const tw_batch* dev, const tw_batch* h, void*
       tk_max = tk > tk_max ? tk : tk_max;
     }
     eng->stitch_layout = stitch_layout(e_max, tk_max);
-    CU(eng->stitch_tables.reserve((size_t)(P > eng->max_units ? P : eng->max_units) + kStitchWarps));
+    CU(stitch_resident_blocks(eng->stitch_layout, eng->n_sm, &stitch_resident));
+  }
+  // unit list of the stitch kernel: at most n / unit_min + 1 units per service.  Every unit pays a
+  // set-up (problem view, bitmap, defaults, cold records), so a large batch takes longer units: about
+  // kStitchUnitsPerWarp per resident warp, which still leaves the queue enough units to end the pass
+  // on a short tail.
+  {
+    const int64_t per_batch = h->n_in_total / ((int64_t)kStitchUnitsPerWarp * stitch_resident * kStitchWarps);
+    eng->unit_min = per_batch > kStitchUnitMin ? (int)per_batch : kStitchUnitMin;
+    int64_t mu = 0;
+    for (int p = 0; p < P; ++p) mu += (h->prob_in_off[p + 1] - h->prob_in_off[p]) / eng->unit_min + 1;
+    if (mu > 0x7fffffff) return fail(TW_ERR_RANGE_LIMIT, "bind: too many stitch units");
+    eng->max_units = (int)mu;
+    CU(eng->unit_prob.reserve((size_t)mu));
+    CU(eng->unit_lo.reserve((size_t)mu));
+    CU(eng->unit_hi.reserve((size_t)mu));
+    CU(eng->unit_count.reserve(2));
+    // the persistent grid: every resident block, or one warp per unit if the list is shorter
+    const int64_t needed = (mu + kStitchWarps - 1) / kStitchWarps;
+    eng->stitch_blocks = (int)(needed < stitch_resident ? needed : stitch_resident);
+    eng->stitch_blocks_max = eng->stitch_blocks;
+    CU(eng->stitch_tables.reserve((size_t)eng->stitch_blocks * kStitchWarps));
   }
   // lists too long for the shared-memory sort of tw_prepare get a slab of global scratch each
   {
@@ -761,11 +775,22 @@ int tw_stitch(tw_engine* eng, const tw_params* params, const uint8_t* cut, const
   tw_params sp;
   rc = scoring_params(eng, params, sp, (cudaStream_t)stream);
   if (rc) return rc;
-  StitchUnits ub{eng->unit_prob.p, eng->unit_lo.p, eng->unit_hi.p, eng->unit_count.p};
+  StitchUnits ub{eng->unit_prob.p, eng->unit_lo.p, eng->unit_hi.p, eng->unit_count.p, eng->unit_count.p + 1};
   CU(launch_stitch(eng->dev, sp, cut, spec, *out, eng->taken.p, eng->taken_words, eng->node_limit, ub,
-                   eng->max_units, eng->stitch_layout, eng->stitch_tables.p, eng->err_flag.p, (cudaStream_t)stream,
-                   eng->launches));
+                   eng->unit_min, eng->stitch_blocks, eng->stitch_layout, eng->stitch_tables.p, eng->err_flag.p,
+                   (cudaStream_t)stream, eng->launches));
   return TW_OK;
+}
+
+// Test hook, not part of the ABI header: run the stitch of the bound batch on `blocks` blocks (1 ..
+// the grid the bind sized), so that one warp takes many units; blocks <= 0 restores the bind's grid.
+// Returns the grid now in effect, or TW_ERR_INVALID.
+int tw_debug_stitch_grid(tw_engine* eng, int blocks) {
+  int rc = need_bound(eng, "tw_debug_stitch_grid");
+  if (rc) return rc;
+  if (blocks > eng->stitch_blocks_max) return fail(TW_ERR_INVALID, "tw_debug_stitch_grid: more blocks than the bind sized");
+  eng->stitch_blocks = blocks > 0 ? blocks : eng->stitch_blocks_max;
+  return eng->stitch_blocks;
 }
 
 int tw_score_assignments(tw_engine* eng, const tw_params* params, const int32_t* assign, const tw_score_out* final_topk,

@@ -24,7 +24,7 @@ constexpr int kWideW = 64;                       // overflow kernel: 2048 candid
 constexpr int kWideThreads = 32;                 // (31 in-spans + carry-in per CTA)
 
 // ---- stitch kernel geometry (tw_stitch.cu) --------------------------------------------------
-constexpr int kStitchWarps = 2;                  // one warp per problem
+constexpr int kStitchWarps = 2;                  // warps per CTA, one unit at a time each
 // Register budget of k_stitch: 14 CTAs = 28 resident warps per SM at 72 registers.  A 64-register
 // budget (32 warps) spills in the hot loop and measured slower on an H100.
 constexpr int kStitchBlocksPerSM = 14;
@@ -98,15 +98,20 @@ struct StitchUnits {
   int32_t* prob;
   int32_t* lo;
   int32_t* hi;
-  int* count;
+  int* count;                                    // units in the list
+  int* next;                                     // queue head of k_stitch, at count + 1 (one memset resets both)
 };
 constexpr int kStitchUnitMin = 48;               // a unit is closed at the first strong cut after this many in-spans
-constexpr int kStitchUnitMaxServices = 4096;     // batches with at least this many services keep one warp per service
-// `tables`: one StitchTables per launched warp (max(n_problems, max_units) + kStitchWarps)
+constexpr int kStitchUnitsPerWarp = 6;           // large batches: longer units, about this many per resident warp
+// blocks of k_stitch resident at once on the device with this slab
+cudaError_t stitch_resident_blocks(const StitchLayout& layout, int n_sm, int* blocks);
+// `unit_min`: shortest unit (tw_api.cu, bind); `blocks`: the persistent grid; `tables`: one
+// StitchTables per warp of the grid (blocks * kStitchWarps)
 cudaError_t launch_stitch(const tw_batch& b, const tw_params& prm, const uint8_t* cut,
                           const tw_score_out& spec, const tw_pass_out& out, uint32_t* taken_words, size_t taken_n_words,
-                          long long node_limit, const StitchUnits& unit_buf, int max_units, const StitchLayout& layout,
-                          StitchTables* tables, int* err_flag, cudaStream_t s, int64_t& launches);
+                          long long node_limit, const StitchUnits& unit_buf, int unit_min, int blocks,
+                          const StitchLayout& layout, StitchTables* tables, int* err_flag, cudaStream_t s,
+                          int64_t& launches);
 constexpr int kSortSmemCap = 16384;               // longest list the shared-memory sort network takes
 cudaError_t launch_sort_ends(const tw_batch& b, int64_t* in_end_sorted, int64_t* out_end_sorted,
                              int max_seg, const int32_t* long_seg, int n_long, int64_t* long_scratch,

@@ -8,11 +8,12 @@
 //   AddAssignment(delete=True)       V1:433-463   -> "taken" bitmap instead of list.remove
 //
 // Window w's candidates exclude out spans consumed by windows < w, so a service is a sequential
-// chain of windows; services are independent.  One WARP owns one service and walks its windows in
-// order: lane l enumerates + scores in-span (window start + l) (a window holds <= 31 in-spans),
-// the candidates meet in shared memory, lanes build the in-span conflict masks in parallel, lane 0
-// runs the exact branch and bound, lanes write assignments and set taken bits.  Parallelism comes
-// from the number of services in the batch (25 000 in the 100 M-span configuration).
+// chain of windows; services are independent, and so are the stretches of a service between strong
+// cuts (k_stitch_units).  One WARP owns one such unit and walks its windows in order: lane l
+// enumerates + scores in-span (window start + l) (a window holds <= 31 in-spans), the candidates meet
+// in shared memory, lanes build the in-span conflict masks in parallel, lane 0 runs the exact branch
+// and bound, lanes write assignments and set taken bits.  A persistent grid of warps takes the units
+// from a queue.
 #include "tw_kernels.cuh"
 
 namespace tw {
@@ -32,6 +33,34 @@ __device__ unsigned long long g_stitch_phase[16];
 #else
 #define TW_SPHASE(k) do { } while (0)
 #define TW_SCOUNT(k, v) do { } while (0)
+#endif
+
+// optional warp timeline (build with -DTW_STITCH_TIMELINE; scripts/stitch_timeline.py reads it): per
+// launched warp the %globaltimer when it starts its first unit and ends its last one, and its SM.  A
+// separate build from the phase timers, whose global atomics would stretch the very tail it measures.
+#ifdef TW_STITCH_TIMELINE
+constexpr int kTimelineCap = 1 << 18;
+__device__ unsigned long long g_stitch_tl[3 * kTimelineCap];   // [warp][start ns, end ns, smid]
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ void timeline_mark(int warp, int lane, bool start) {
+  if (lane != 0 || warp >= kTimelineCap) return;
+  const unsigned long long t = global_ns();
+  if (start) {
+    unsigned sm;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    if (g_stitch_tl[3 * warp] == 0) g_stitch_tl[3 * warp] = t;
+    g_stitch_tl[3 * warp + 2] = sm;
+  } else {
+    g_stitch_tl[3 * warp + 1] = t;
+  }
+}
+#define TW_TIMELINE(warp, start) timeline_mark((warp), lane, (start))
+#else
+#define TW_TIMELINE(warp, start) do { } while (0)
 #endif
 
 __device__ __forceinline__ void prefetch_l1(const void* p) {
@@ -481,29 +510,12 @@ __device__ __noinline__ long long stitch_mwis_large(PackedWindowBuf& wb, StitchT
   return nodes;
 }
 
-__global__ void __launch_bounds__(kStitchWarps * 32, kStitchBlocksPerSM)
-k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_score_out spec, tw_pass_out out,
-         uint32_t* __restrict__ taken, long long node_limit, StitchUnits units, StitchLayout layout,
-         StitchTables* __restrict__ tables, int* __restrict__ err_flag) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  __shared__ double etab[64];
-  load_exp_table(etab);
-  const int warp_in_block = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  // one warp = one UNIT: a stretch [u0, u1) of one service's in-spans that shares no candidate span with
-  // the rest of the service (k_stitch_units), or the whole service when no unit list was built
-  const int u = blockIdx.x * kStitchWarps + warp_in_block;
-  int p, u0 = 0, u1 = -1;
-  if (units.prob) {
-    if (u >= *units.count) return;
-    p = units.prob[u];
-    u0 = units.lo[u];
-    u1 = units.hi[u];
-  } else {
-    p = u;
-    if (p >= b.n_problems) return;
-  }
-  const StitchSlab slab{smem_raw + warp_in_block * layout.bytes};
+// One UNIT of the stitch by one warp: in-spans [u0, u1) of service p (u1 < 0: to the end of the service).
+__device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& prm, const uint8_t* __restrict__ cut_all,
+                                            const tw_score_out& spec, const tw_pass_out& out, uint32_t* __restrict__ taken,
+                                            long long node_limit, const StitchLayout& layout, StitchTables& tb,
+                                            int* __restrict__ err_flag, const StitchSlab& slab, const double* etab,
+                                            int lane, int p, int u0, int u1) {
   StitchWarpSmem& sm = slab.fixed();
 #ifdef TW_PROFILE_PHASES
   long long _sp_t0 = clock64();
@@ -745,7 +757,7 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
     const unsigned slow_mask = __ballot_sync(0xffffffffu, active && !fast);   // (all lanes vote: the counter macro runs on lane 0 only)
     TW_SCOUNT(14, __popc(slow_mask));
     if (slow_mask)
-      stitch_search_lanes(v, wb, tables[u], prm, out, tk_base, w, gauss_base, mix_base, etab, E, lane, ws, i, in_s, in_e,
+      stitch_search_lanes(v, wb, tb, prm, out, tk_base, w, gauss_base, mix_base, etab, E, lane, ws, i, in_s, in_e,
                           active && !fast, batch0);
     __syncwarp();
     TW_SPHASE(6);                                // slow path
@@ -758,7 +770,7 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
       if (nw <= kSmallWindow) solved = stitch_small_window(sm, wb, E, nw, lane, &nodes);
       if (!solved) {
         TW_SCOUNT(15, 1);
-        nodes = stitch_mwis_large(wb, tables[u], E, nw, node_limit, lane);
+        nodes = stitch_mwis_large(wb, tb, E, nw, node_limit, lane);
       }
     }
     __syncwarp();
@@ -792,6 +804,41 @@ k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_scor
       atomicMax(&out.counters[p * 4 + 2], (int)(max_nodes > 0x7fffffffLL ? 0x7fffffffLL : max_nodes));
       atomicMin(&out.counters[p * 4 + 3], rc);
     }
+  }
+}
+
+// Persistent grid (launch_stitch: as many warps as can be resident): every warp takes units from the
+// queue head `units.next` until the list is empty, so no warp slot idles while units remain, and the
+// tail of a pass is the length of one unit, not of one service.
+__global__ void __launch_bounds__(kStitchWarps * 32, kStitchBlocksPerSM)
+k_stitch(tw_batch b, tw_params prm, const uint8_t* __restrict__ cut_all, tw_score_out spec, tw_pass_out out,
+         uint32_t* __restrict__ taken, long long node_limit, StitchUnits units, StitchLayout layout,
+         StitchTables* __restrict__ tables, int* __restrict__ err_flag) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  __shared__ double etab[64];
+  load_exp_table(etab);
+  const int warp_in_block = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int slot = blockIdx.x * kStitchWarps + warp_in_block;
+  const StitchSlab slab{smem_raw + warp_in_block * layout.bytes};
+  StitchTables& tb = tables[slot];
+  // unit u: in-spans [lo[u], hi[u]) of service prob[u] (k_stitch_units), or the whole service u when
+  // no unit list was built
+  const int n_units = units.prob ? *units.count : b.n_problems;
+  while (true) {
+    int u = 0;
+    if (lane == 0) u = atomicAdd(units.next, 1);
+    u = __shfl_sync(0xffffffffu, u, 0);
+    if (u >= n_units) break;
+    int p = u, u0 = 0, u1 = -1;
+    if (units.prob) {
+      p = units.prob[u];
+      u0 = units.lo[u];
+      u1 = units.hi[u];
+    }
+    TW_TIMELINE(slot, true);
+    stitch_unit(b, prm, cut_all, spec, out, taken, node_limit, layout, tb, err_flag, slab, etab, lane, p, u0, u1);
+    TW_TIMELINE(slot, false);
   }
 }
 
@@ -888,6 +935,19 @@ extern "C" int tw_debug_stitch_phases(unsigned long long* out16, int reset) {
 }
 #endif
 
+#ifdef TW_STITCH_TIMELINE
+// out: [kTimelineCap][3] (start ns, end ns, smid) of every launched warp; zero where no warp ran
+extern "C" int tw_debug_stitch_timeline(unsigned long long* out, int cap, int reset) {
+  if (cap < kTimelineCap) return -1;
+  if (cudaMemcpyFromSymbol(out, g_stitch_tl, sizeof(g_stitch_tl)) != cudaSuccess) return -2;
+  void* dev = nullptr;
+  if (reset && (cudaGetSymbolAddress(&dev, g_stitch_tl) != cudaSuccess ||
+                cudaMemset(dev, 0, sizeof(g_stitch_tl)) != cudaSuccess))
+    return -2;
+  return kTimelineCap;
+}
+#endif
+
 StitchLayout stitch_layout(int e_max, int tk_words_max) {
   StitchLayout L;
   L.tk_words = tk_words_max < kTakenWords ? tk_words_max : kTakenWords;
@@ -901,33 +961,37 @@ cudaError_t setup_stitch() {   // the largest slab any batch can ask for
                               stitch_layout(TW_MAX_E, kTakenWords).bytes * kStitchWarps);
 }
 
+cudaError_t stitch_resident_blocks(const StitchLayout& layout, int n_sm, int* blocks) {
+  int per_sm = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_stitch, kStitchWarps * 32,
+                                                                      (size_t)layout.bytes * kStitchWarps);
+  *blocks = (per_sm > 0 ? per_sm : 1) * n_sm;
+  return e;
+}
+
 cudaError_t launch_stitch(const tw_batch& b, const tw_params& prm, const uint8_t* cut,
                           const tw_score_out& spec, const tw_pass_out& out, uint32_t* taken_words, size_t taken_n_words,
-                          long long node_limit, const StitchUnits& unit_buf, int max_units, const StitchLayout& layout,
-                          StitchTables* tables, int* err_flag, cudaStream_t s, int64_t& launches) {
+                          long long node_limit, const StitchUnits& unit_buf, int unit_min, int blocks,
+                          const StitchLayout& layout, StitchTables* tables, int* err_flag, cudaStream_t s,
+                          int64_t& launches) {
   cudaError_t e = cudaMemsetAsync(taken_words, 0, taken_n_words * sizeof(uint32_t), s);
   if (e != cudaSuccess) return e;
   if (out.counters) {
     e = cudaMemsetAsync(out.counters, 0, (size_t)b.n_problems * 4 * sizeof(int32_t), s);
     if (e != cudaSuccess) return e;
   }
-  const size_t smem = (size_t)layout.bytes * kStitchWarps;
-  StitchUnits units{nullptr, nullptr, nullptr, nullptr};
-  int warps = b.n_problems;
-  // Units pay when services alone cannot fill the machine (a shipped directory has 2-6 services; the
-  // 132 SMs of an H100 hold ~2500 stitch warps); with thousands of services one warp per service is
-  // already enough parallelism and the unit pre-pass + per-unit set-up cost more than the shorter tail
-  // gains.  The maps of the scoring kernel prove which cuts are strong.
-  if (spec.used_lo && unit_buf.prob && max_units > 0 && b.n_problems < kStitchUnitMaxServices) {
-    units = unit_buf;
-    e = cudaMemsetAsync(units.count, 0, sizeof(int), s);
-    if (e != cudaSuccess) return e;
-    k_stitch_units<<<(b.n_problems + 3) / 4, 128, 0, s>>>(b, cut, spec, kStitchUnitMin, units);
+  // count and queue head are adjacent: one memset resets both
+  e = cudaMemsetAsync(unit_buf.count, 0, 2 * sizeof(int), s);
+  if (e != cudaSuccess) return e;
+  StitchUnits units = unit_buf;
+  if (spec.used_lo) {   // the maps of the scoring kernel prove which cuts are strong
+    k_stitch_units<<<(b.n_problems + 3) / 4, 128, 0, s>>>(b, cut, spec, unit_min, units);
     e = after_launch(launches);
     if (e != cudaSuccess) return e;
-    warps = max_units;
+  } else {
+    units.prob = units.lo = units.hi = nullptr;   // one unit per service
   }
-  int blocks = (warps + kStitchWarps - 1) / kStitchWarps;
+  const size_t smem = (size_t)layout.bytes * kStitchWarps;
   k_stitch<<<blocks, kStitchWarps * 32, smem, s>>>(b, prm, cut, spec, out, taken_words, node_limit, units, layout,
                                                    tables, err_flag);
   return after_launch(launches);
