@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define TW_ABI_VERSION 6
+#define TW_ABI_VERSION 7
 
 /* Algorithm constants hard-coded by the reference. */
 #define TW_MAX_E 8             /* engine limit on out-eps per service (shipped data: <= 4)      */
@@ -424,6 +424,30 @@ int tw_find_order(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc
 int tw_accuracy(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc, const int32_t* truth,
                 const int32_t* assign, const int32_t* topk_idx, const uint8_t* topk_cnt, const int32_t* in_trace,
                 int32_t n_traces, const uint8_t* prob_first, uint64_t* per_prob_out, uint64_t* e2e_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * End-to-end request trees (ConstructEndToEndTraces, helpers/utils.py:216, called from executor.py:1210-1230).
+ * The nodes of a batch are its spans: in-span g (global index) is node g, out-span j (global index) is node
+ * n_in_total + j.  Parents:
+ *   out-span j of callee e of service p: in-span i of p iff assign[tuple_off[p] + e*n_p + i] == j (the layout of
+ *     tw_pass_out.assign: an engine result, tw_ground_truth's, another predictor's; codes < 0 give no child);
+ *   in-span g: in_caller[g], the out-span node of the client span of the RPC whose server side it is (observed,
+ *     from the spans' own references), -1 when that span is not in the batch.
+ * A node without a parent is a root: an in-span root is a reconstructed request, an out-span root the top of a
+ * detached fragment (an out-span no in-span took).  Per node, all DEVICE int32 [n_in_total + n_out_total]:
+ *   parent_out[x]  the parent node or -1
+ *   root_out[x]    the root of x, found by ceil(log2 n_nodes) + 1 rounds of pointer jumping (a round after one
+ *                  that moved no node returns at once); -1 when x lies on or under a cycle of links
+ *   size_out[r]    number of nodes whose root is r (0 for a non-root)
+ * Takes the offsets of `dev` / `host_desc` (skip budgets allowed; span arrays, term tables not read) and does not
+ * touch a bound batch.  TW_ERR_INVALID when an out-span is the child of two in-spans, two in-spans name the same
+ * caller, an assign index lies outside its callee's list or a caller is not an out-span node (tw_last_error()
+ * names the smallest such node); TW_ERR_RANGE_LIMIT when n_in_total + n_out_total >= 2^31.  Blocks until
+ * `stream` is idle.  Trace ids are not read: the trees come from the links alone.
+ * ---------------------------------------------------------------------------------------------- */
+int tw_assemble_traces(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc, const int32_t* assign,
+                       const int32_t* in_caller, int32_t* parent_out, int32_t* root_out, int32_t* size_out,
+                       void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,6 +1,7 @@
 """Reconstruct a directory of Jaeger JSON traces end to end: loader -> batch engine -> accuracy.
 
     python scripts/reconstruct_traces.py <trace dir> [--layout hotel|media|node|alibaba] [--device 0] [--likelihood]
+                                         [--traces FILE.npz]
 
 Prints, per solved service, the assignment accuracy against the traces' own parent links
 (the reference's AccuracyForService, helpers/utils.py:34-60) and the time of each stage — the same
@@ -8,7 +9,11 @@ numbers executor.py prints for `--predictor_indices 10`.  --likelihood adds, per
 log-likelihood of the chosen tuples under the refitted delay model, quantiles of the margin to the runner-up
 (or to the best tuple, for an in-span that did not get its best), and for the wrong in-spans whether the
 true tuple scores above the chosen one (a search error: the window's MWIS and deletion pushed it out),
-below it (a model error), or is infeasible."""
+below it (a model error), or is infeasible.  --traces joins the assignments into end-to-end request trees on
+the device (BatchSolver.assemble) and writes them to FILE.npz: parent, root, size per node (in-span g is node
+g, out-span j node n_in + j), exact per in-span (1 / 0 for a reconstructed request that is / is not exactly its
+trace, -1 for an in-span that is not a root) and the node -> (trace id, span id) tables node_trace_id,
+node_span_id; it prints the share of exact requests beside the end-to-end accuracy."""
 import argparse, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -19,10 +24,11 @@ ap.add_argument("--layout", default="hotel", choices=["hotel", "media", "node", 
 ap.add_argument("--device", type=int, default=0)
 ap.add_argument("--seed", type=int, default=10)
 ap.add_argument("--likelihood", action="store_true", help="print per-service confidence and error classes")
+ap.add_argument("--traces", default=None, metavar="FILE.npz", help="write the reconstructed request trees")
 args = ap.parse_args()
 
 from traceweaver_b200.api import BatchSolver
-from traceweaver_b200.loader import load_jaeger_dir, to_host_batch, accuracy
+from traceweaver_b200.loader import load_jaeger_dir, to_host_batch, accuracy, end_to_end_accuracy
 
 t0 = time.perf_counter()
 from traceweaver_b200.engine import Engine
@@ -63,3 +69,22 @@ for p, s in enumerate(ok):
           f"single-candidate {int(np.isinf(m).sum())}  wrong {int(wrong.sum())}: search error "
           f"{int((feas & (ts > cs)).sum())}, model error {int((feas & (ts <= cs)).sum())}, "
           f"truth infeasible {int((~feas).sum())}")
+if args.traces:
+    from traceweaver_b200 import traces
+    in_caller = traces.caller_links(ok, hb)
+    truth_all = np.concatenate([s.truth.reshape(-1) for s in ok]).astype(np.int32)
+    t4 = time.perf_counter()
+    tr = solver.assemble(hb, np.array(out["assign"]), in_caller, truth=truth_all)
+    t5 = time.perf_counter()
+    ids = [i for s in ok for i in s.in_ids] + [i for s in ok for ids in s.out_ids for i in ids]
+    np.savez(args.traces, parent=tr["parent"], root=tr["root"], size=tr["size"], exact=tr["exact"],
+             node_trace_id=np.array([t for t, _ in ids]), node_span_id=np.array([sid for _, sid in ids]))
+    n_in = int(hb.prob_in_off[-1])
+    requests = int((tr["exact"] >= 0).sum())
+    e2e = end_to_end_accuracy([[t for t, _ in s.in_ids] for s in ok], [s.truth for s in ok],
+                              [out["assign"][int(hb.prob_tuple_off[p]):int(hb.prob_tuple_off[p + 1])]
+                               for p in range(len(ok))])
+    print(f"request trees ({1e3 * (t5 - t4):.2f} ms, with the truth join): {requests} requests, "
+          f"{int((tr['size'][n_in:] > 0).sum())} detached fragments, {int((tr['root'] < 0).sum())} nodes on cycles; "
+          f"exact {100 * (tr['exact'] == 1).sum() / max(requests, 1):7.3f} %  end-to-end accuracy {100 * e2e:7.3f} %"
+          f"  -> {args.traces}")

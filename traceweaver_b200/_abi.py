@@ -4,7 +4,7 @@ Field order and widths must match the header exactly; tests/test_abi.py checks s
 against values compiled from the header."""
 import ctypes as C
 
-TW_ABI_VERSION = 6
+TW_ABI_VERSION = 7
 TW_SCORE_KEEP_WINDOWS = 1
 TW_MAX_E = 8
 TW_K = 5

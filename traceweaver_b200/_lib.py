@@ -53,6 +53,8 @@ SYMBOLS = {
                               C.c_void_p]),
     "tw_build_dist_samples": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                         C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tw_assemble_traces": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch), C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
 }
 
 

@@ -244,3 +244,20 @@ class BatchSolver:
         eng.status()
         return dict(score=lk["score"].cpu().numpy(), code=lk["code"].cpu().numpy(),
                     service_loglik=lk["prob_sum"].cpu().numpy(), service_codes=lk["prob_count"].cpu().numpy())
+
+    def assemble(self, hb: HostBatch, assign, in_caller, truth=None):
+        """End-to-end request trees of the whole batch `hb` (tw_assemble_traces; whatever grouping solve()
+        used): `assign` in the layout of out["assign"], `in_caller` from traces.caller_links.  Host arrays
+        over the nodes (in-span g is node g, out-span j node n_in + j): parent, root (-1 on or under a cycle),
+        size (nodes per root).  With `truth` (an assignment in the same layout, e.g. the loader's ground
+        truth) also exact [n_in], int8: for an in-span root r, 1 iff the request rooted at r holds exactly the
+        nodes it holds under the truth; -1 for an in-span that is not a root."""
+        from . import traces
+        eng = self.engine
+        links = _to_device(dict(in_caller=np.asarray(in_caller, np.int32).reshape(-1)), eng.device)["in_caller"]
+        res = traces.assemble(eng, hb, assign, links)
+        out = {k: v.cpu().numpy() for k, v in res.items()}
+        if truth is not None:
+            ref = traces.assemble(eng, hb, truth, links)
+            out["exact"] = traces.exact_requests(res["root"], ref["root"], int(hb.prob_in_off[-1])).cpu().numpy()
+        return out

@@ -97,6 +97,11 @@ struct tw_engine {
   DevBuf<int> order_missing;
   DevBuf<uint8_t> acc_flags;
   DevBuf<unsigned long long> acc_first;
+  // request trees (tw_assemble_traces): caller claim words, error words + per-round flags, and what the
+  // last call did (tw_debug_trace_rounds)
+  DevBuf<int32_t> trace_claim;
+  DevBuf<int32_t> trace_flags;
+  int trace_rounds_launched = 0, trace_rounds_run = 0;
   // skip / cache mode scratch (tw_skip_solve)
   DevBuf<uint32_t> skip_sets;
   DevBuf<int64_t> skip_set_off;
@@ -688,6 +693,54 @@ int tw_accuracy(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const in
   CU(launch_accuracy(*dev, truth, assign, topk_idx, topk_cnt, n_traces ? in_trace : nullptr, eng->in_prob.p, prob_first,
                      n_traces, (unsigned long long*)per_prob_out, eng->acc_flags.p, eng->acc_first.p,
                      (unsigned long long*)e2e_out, s, eng->launches));
+  return TW_OK;
+}
+
+int tw_assemble_traces(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const int32_t* assign,
+                       const int32_t* in_caller, int32_t* parent_out, int32_t* root_out, int32_t* size_out,
+                       void* stream_) {
+  if (!eng || !dev || !assign || !in_caller || !parent_out || !root_out || !size_out)
+    return fail(TW_ERR_INVALID, "tw_assemble_traces: NULL argument");
+  int rc = validate_host(h, "tw_assemble_traces", false, true);
+  if (rc) return rc;
+  const int64_t n_in = h->n_in_total, n_out = h->n_out_total, n_nodes = n_in + n_out;
+  if (n_nodes >= ((int64_t)1 << 31))
+    return fail(TW_ERR_RANGE_LIMIT, "tw_assemble_traces: %s nodes do not fit int32 node ids",
+                std::to_string(n_nodes).c_str());
+  cudaStream_t s = (cudaStream_t)stream_;
+  CU(cudaSetDevice(eng->device));
+  const int rounds = trace_rounds(n_nodes);
+  CU(eng->trace_claim.reserve((size_t)n_out));
+  CU(eng->trace_flags.reserve((size_t)(4 + rounds)));
+  int32_t* err = eng->trace_flags.p;
+  int* changed = (int*)(eng->trace_flags.p + 4);
+  CU(launch_assemble_traces(*dev, h->prob_tuple_off[h->n_problems], assign, in_caller, parent_out, root_out, size_out,
+                            eng->trace_claim.p, err, changed, rounds, eng->n_sm, s, eng->launches));
+  std::vector<int32_t> flags((size_t)(4 + rounds));
+  CU(cudaMemcpyAsync(flags.data(), err, flags.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  eng->trace_rounds_launched = rounds;
+  eng->trace_rounds_run = 1;                               // round r > 0 runs iff round r - 1 moved a node
+  while (eng->trace_rounds_run < rounds && flags[4 + eng->trace_rounds_run - 1]) ++eng->trace_rounds_run;
+  const int32_t none = 0x7f7f7f7f;
+  const char* what[4] = {"out-span node %s is the child of two in-spans%s",
+                         "out-span node %s is the caller of two in-spans%s",
+                         "in-span node %s has a child index outside its callee's list%s",
+                         "in-span node %s has a caller that is not an out-span node%s"};
+  for (int k : {3, 1, 2, 0})                               // the callers first, as traces.parents_host
+    if (flags[k] != none) {
+      const std::string msg = std::string("tw_assemble_traces: ") + what[k];
+      return fail(TW_ERR_INVALID, msg.c_str(), std::to_string(flags[k]).c_str(), "");
+    }
+  return TW_OK;
+}
+
+// Test hook, not part of the ABI header: pointer-jumping rounds the last tw_assemble_traces launched and
+// the rounds of them that ran (the others returned at once after a round that moved no node).
+int tw_debug_trace_rounds(tw_engine* eng, int* launched, int* run) {
+  if (!eng || !launched || !run) return fail(TW_ERR_INVALID, "tw_debug_trace_rounds: NULL argument");
+  *launched = eng->trace_rounds_launched;
+  *run = eng->trace_rounds_run;
   return TW_OK;
 }
 

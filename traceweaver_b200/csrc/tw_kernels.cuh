@@ -252,4 +252,13 @@ cudaError_t launch_accuracy(const tw_batch& b, const int32_t* truth, const int32
                             unsigned long long* trace_first, unsigned long long* out4, cudaStream_t s,
                             int64_t& launches);
 
+// tw_traces.cu: pointer-jumping rounds for n_nodes nodes, ceil(log2 n_nodes) + 1, and the launches of
+// tw_assemble_traces.  claim: [n_out] scratch; err: 4 words (twice-claimed out-span, twice-named caller,
+// in-span with an assign index out of range, in-span whose caller is not an out-span node: the smallest
+// such node, 0x7f7f7f7f = none); changed: [rounds] flags, round r moved some node.
+int trace_rounds(int64_t n_nodes);
+cudaError_t launch_assemble_traces(const tw_batch& b, int64_t n_tuple, const int32_t* assign, const int32_t* in_caller,
+                                   int32_t* parent, int32_t* root, int32_t* size, int32_t* claim, int32_t* err,
+                                   int* changed, int rounds, int n_sm, cudaStream_t s, int64_t& launches);
+
 }  // namespace tw

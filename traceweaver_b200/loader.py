@@ -54,6 +54,10 @@ class ServiceProblem:
     out_ids: List[List[tuple]]       # per ep (topological order)
     truth: np.ndarray                # int32 [E, n], -1 where the trace has no such child
     graph_edges: List[tuple] = field(default_factory=list)
+    # per in-span: (trace id, span id) of the client span of its RPC (the span it references, or the client
+    # twin a rewrite gave it), None for a request that enters here.  The observed links of the request trees
+    # (traces.caller_links); an id is a span reference, which names the trace as well as the span.
+    in_caller_ids: List[Optional[tuple]] = field(default_factory=list)
 
 
 def _span_kind(span):
@@ -88,14 +92,15 @@ class _Rows:
     """Growing SoA of one service's spans of one kind (server or client)."""
 
     def __init__(self):
-        self.start, self.dur, self.tid, self.sid, self.other = [], [], [], [], []
+        self.start, self.dur, self.tid, self.sid, self.other, self.caller = [], [], [], [], [], []
 
-    def add(self, start, dur, tid, sid, other):
+    def add(self, start, dur, tid, sid, other, caller=None):
         self.start.append(start)
         self.dur.append(dur)
         self.tid.append(tid)
         self.sid.append(sid)
         self.other.append(other)
+        self.caller.append(caller)
 
 
 def _nodes_plain(d, path):
@@ -322,7 +327,8 @@ def load_jaeger_dir(directory: str, first_span: Optional[str] = HOTEL_FIRST_SPAN
                 outs.setdefault(me, _Rows()).add(start, dur, tid, sid, nodes[children[k][0]][5])   # GetChildProcess
             elif kind == "server":
                 other = "client_" + op if par < 0 else nodes[par][5]                      # GetParentProcess
-                ins.setdefault(me, _Rows()).add(start, dur, tid, sid, other)
+                caller = (nodes[par][0], nodes[par][1]) if par >= 0 and nodes[par][6] == "client" else None
+                ins.setdefault(me, _Rows()).add(start, dur, tid, sid, other, caller)
             else:
                 raise ValueError(f"{path}: span.kind {kind!r} (executor.py:819)")
             stack.extend(reversed(children[k]))
@@ -423,7 +429,8 @@ def _finish_service(L, truth_given, violated) -> ServiceProblem:
         name=L["process"], in_ep=L["in_ep"], out_eps_given=given, out_eps=topo, problem=prob,
         in_ids=[(i_rows.tid[k], i_rows.sid[k]) for k in in_idx],
         out_ids=[[(o_rows.tid[k], o_rows.sid[k]) for k in ix] for ix in out_idx],
-        truth=np.ascontiguousarray(np.asarray(truth_given)[g_of]), graph_edges=list(G.edges()))
+        truth=np.ascontiguousarray(np.asarray(truth_given)[g_of]), graph_edges=list(G.edges()),
+        in_caller_ids=[i_rows.caller[k] for k in in_idx])
 
 
 def _service_problem(process, i_rows: _Rows, o_rows: _Rows) -> Optional[ServiceProblem]:

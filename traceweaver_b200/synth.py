@@ -169,6 +169,74 @@ def alibaba_stream(n_services: int = 2000, n_in: int = 1250, compress=(1, 200, 1
     return blocks
 
 
+def _sort_rows(start, end):
+    """Rows sorted by (start, end): sorted copies and rank[s, r] = position of element r in row s."""
+    order = np.lexsort((end, start), axis=-1)
+    rank = np.empty_like(order)
+    np.put_along_axis(rank, order, np.arange(order.shape[1])[None, :], axis=1)
+    return np.take_along_axis(start, order, axis=1), np.take_along_axis(end, order, axis=1), rank
+
+
+def hotel_tree(n_replicas: int, n_req: int = 1000, load: float = 100.0, seed: int = 10):
+    """Requests of a two-tier hotel_reservation-shaped deployment, for the request trees (traces.py).  Each of
+    `n_replicas` replicas gets `n_req` requests at its frontend, which calls search, then reservation, then
+    profile (the hotel_frontend DAG); search calls geo, then rate (hotel_search).  Frontend and search are the
+    solved services; every server span lies inside its client span (a network hop of a few tens of us each
+    way).  Returns dict(blocks=[frontend, search] ServiceBlocks, hb (frontend problems, then search problems),
+    in_caller: int32 [n_in] node ids as traces.caller_links gives them, truth: the true assignment,
+    in_request: int32 [n_in] the request every in-span serves, numbered replica * n_req + arrival)."""
+    rng = np.random.default_rng(seed)
+    S, n = n_replicas, n_req
+    lat = lambda: _lognormal(rng, 40, 0.5, (S, n))
+    ia = np.maximum(np.rint(rng.exponential(INTERARRIVAL_US_AT_LOAD_100 * 100.0 / load, size=(S, n))), 1).astype(np.int64)
+    f_start = T0 + np.cumsum(ia, axis=1)
+    c0s = f_start + _lognormal(rng, 270, 0.6, (S, n))                 # frontend -> search (client)
+    s_start = c0s + lat()                                               # search (server)
+    geo_s = s_start + _lognormal(rng, 267, 0.6, (S, n))
+    geo_e = geo_s + _lognormal(rng, 3700, 0.5, (S, n))
+    rate_s = geo_e + _lognormal(rng, 165, 0.8, (S, n))
+    rate_e = rate_s + _lognormal(rng, 7300, 0.6, (S, n))
+    s_end = rate_e + _lognormal(rng, 68, 0.8, (S, n))
+    c0e = s_end + lat()
+    res_s = c0e + _lognormal(rng, 195, 0.7, (S, n))
+    res_e = res_s + _lognormal(rng, 7300, 1.2, (S, n))
+    pro_s = res_e + _lognormal(rng, 210, 0.6, (S, n))
+    pro_e = pro_s + _lognormal(rng, 4150, 0.55, (S, n))
+    f_end = pro_e + _lognormal(rng, 165, 0.7, (S, n))
+
+    def block(in_s, in_e, calls, preds, name):
+        in_s, in_e, in_rank = _sort_rows(in_s, in_e)
+        out_s, out_e, ranks = [], [], []
+        truth = np.empty((len(calls), S, n), np.int32)
+        for e, (cs, ce) in enumerate(calls):
+            a, b, rk = _sort_rows(cs, ce)
+            out_s.append(a)
+            out_e.append(b)
+            ranks.append(rk)
+            np.put_along_axis(truth[e], in_rank, rk, axis=1)             # in-span of request r -> its call
+        return ServiceBlock(in_start=in_s, in_end=in_e, out_start=out_s, out_end=out_e, preds=preds, truth=truth,
+                            name=name), in_rank, ranks
+
+    front, _, f_ranks = block(f_start, f_end, [(c0s, c0e), (res_s, res_e), (pro_s, pro_e)], [[], [0], [0, 1]],
+                              f"hotel_tree_frontend@load{load:g}")
+    search, s_rank, _ = block(s_start, s_end, [(geo_s, geo_e), (rate_s, rate_e)], [[], [0]],
+                              f"hotel_tree_search@load{load:g}")
+    from .batch import build_batch_from_blocks
+    hb = build_batch_from_blocks([front, search])
+    n_in = 2 * S * n
+    rows = np.arange(S)[:, None]
+    in_caller = np.empty((S, n), np.int32)
+    # search in-span of request r (node S*n + s*n + rank) <- the frontend's call to search (ep 0 of problem s)
+    in_caller[rows, s_rank] = n_in + (rows * 3) * n + f_ranks[0]
+    in_caller = np.concatenate([np.full(S * n, -1, np.int32), in_caller.reshape(-1)])
+    request = (rows * n + np.arange(n)[None, :]).astype(np.int32)      # request number of (replica, arrival)
+    in_request = np.empty((2, S, n), np.int32)
+    in_request[0] = request                                             # frontend arrivals are in start order
+    in_request[1][rows, s_rank] = request
+    return dict(blocks=[front, search], hb=hb, in_caller=in_caller, truth=truth_assign([front, search]),
+                in_request=in_request.reshape(-1))
+
+
 def span_count(blocks):
     return int(sum(b.in_start.size * (1 + len(b.out_start)) for b in blocks))
 
