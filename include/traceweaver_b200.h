@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define TW_ABI_VERSION 7
+#define TW_ABI_VERSION 8
 
 /* Algorithm constants hard-coded by the reference. */
 #define TW_MAX_E 8             /* engine limit on out-eps per service (shipped data: <= 4)      */
@@ -448,6 +448,54 @@ int tw_accuracy(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc, 
 int tw_assemble_traces(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc, const int32_t* assign,
                        const int32_t* in_caller, int32_t* parent_out, int32_t* root_out, int32_t* size_out,
                        void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Critical paths of the reconstructed requests: where each request's time went.  This project's own
+ * definition (the reference's consumers of its traces are not part of it).  Nodes and links are those of
+ * tw_assemble_traces; a node's interval is [start, end] of its span (the float64 times when dev_times_f64
+ * is given, else the int64 times of `dev`; a span with end < start counts as empty).  A request is an
+ * in-span root r; its window is [start_r, max(start_r, end_r)], its latency the window's length.  Windows
+ * are handed down the tree; every node that gets one is on the path, and its self time is the part of its
+ * window it hands to no child:
+ *   in-span with window [a, b]: each child out-span (callee position e) is clipped to [a, b] and eligible
+ *     iff what is left, [s_k, e_k], is not empty.  From c = b backwards, the unchosen eligible child with
+ *     s_k < c and the largest min(e_k, c) (lowest e on a tie) gets [s_k, min(e_k, c)]; c - min(e_k, c) is
+ *     self time and c becomes s_k.  When no child qualifies, c - a is self time.
+ *   out-span with window [a, b]: its child in-span (the in-span whose caller it is) is on the path iff
+ *     its interval clipped to [a, b] is not empty, and gets that window; the rest of [a, b] is self time
+ *     (network, queueing, or the whole callee when its server span is not in the batch).
+ * Over the on-path nodes of a request the self times add up to its latency (exactly for int64 times).
+ * Outputs, all DEVICE buffers of the caller (N = n_in_total + n_out_total):
+ *   root       int32 [N]        as tw_assemble_traces' root_out
+ *   on_path    uint8 [N]        1 iff the node is on its request's path
+ *   self_us    double [N]       self time, 0 off the path
+ *   culprit    int32 [n_in]     for a request root: its on-path node with the largest self time (smallest
+ *                               node id on a tie); -1 for any other in-span
+ *   server_us, server_visits    double / int32 [P][2]: self time and count of the on-path in-spans of
+ *                               service p, column 0 over all requests, column 1 over the requests whose
+ *                               latency is >= slow_us
+ *   call_us    double [n_ep][2] self time of the on-path out-spans of global callee ep, same columns
+ *   requests   int32 [2]        requests in each column
+ * The sums are fixed-order reductions: bit-identical from run to run.  The join runs inside (limits and
+ * TW_ERR_INVALID / TW_ERR_RANGE_LIMIT errors of tw_assemble_traces, which it reads back); then one launch
+ * per level of in-spans, as many as the join's pointer-jumping rounds allow for the depth of the trees
+ * (at most 64), two culprit launches and one reduction.  In-spans deeper than the last level are walked by
+ * its threads one after another; a tree too deep even for that sets TW_ERR_RANGE_LIMIT in the engine's
+ * device status (tw_engine_status).  A bound batch is not touched.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct tw_critical_out {
+  int32_t* root;
+  uint8_t* on_path;
+  double* self_us;
+  int32_t* culprit;
+  double* server_us;
+  int32_t* server_visits;
+  double* call_us;
+  int32_t* requests;
+} tw_critical_out;
+int tw_critical_paths(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc,
+                      const tw_times_f64* dev_times_f64, const int32_t* assign, const int32_t* in_caller,
+                      double slow_us, const tw_critical_out* out, void* stream);
 
 #ifdef __cplusplus
 }

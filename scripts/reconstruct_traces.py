@@ -13,7 +13,12 @@ below it (a model error), or is infeasible.  --traces joins the assignments into
 the device (BatchSolver.assemble) and writes them to FILE.npz: parent, root, size per node (in-span g is node
 g, out-span j node n_in + j), exact per in-span (1 / 0 for a reconstructed request that is / is not exactly its
 trace, -1 for an in-span that is not a root) and the node -> (trace id, span id) tables node_trace_id,
-node_span_id; it prints the share of exact requests beside the end-to-end accuracy."""
+node_span_id; it prints the share of exact requests beside the end-to-end accuracy.  --critical-path
+(BatchSolver.critical_paths; definition in traceweaver_b200/traces.py) prints, per service and per callee
+edge, the share of the requests' critical time spent there, over all requests and over the slow ones (latency at
+or above the --slow-quantile of all latencies), on the predicted assignment and on the truth, and the largest
+difference between the two; the services the slow requests' culprits belong to; and the share of exact requests
+per latency decile.  With --traces the file also holds on_path, self_us and culprit of the prediction."""
 import argparse, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -25,6 +30,8 @@ ap.add_argument("--device", type=int, default=0)
 ap.add_argument("--seed", type=int, default=10)
 ap.add_argument("--likelihood", action="store_true", help="print per-service confidence and error classes")
 ap.add_argument("--traces", default=None, metavar="FILE.npz", help="write the reconstructed request trees")
+ap.add_argument("--critical-path", action="store_true", help="print where the requests' time went")
+ap.add_argument("--slow-quantile", type=float, default=0.99, help="latency quantile of the slow requests")
 args = ap.parse_args()
 
 from traceweaver_b200.api import BatchSolver
@@ -69,6 +76,46 @@ for p, s in enumerate(ok):
           f"single-candidate {int(np.isinf(m).sum())}  wrong {int(wrong.sum())}: search error "
           f"{int((feas & (ts > cs)).sum())}, model error {int((feas & (ts <= cs)).sum())}, "
           f"truth infeasible {int((~feas).sum())}")
+cp = None
+if args.critical_path:
+    from traceweaver_b200 import traces
+    in_caller = traces.caller_links(ok, hb)
+    truth_all = np.concatenate([s.truth.reshape(-1) for s in ok]).astype(np.int32)
+    t4 = time.perf_counter()
+    cp = solver.critical_paths(hb, np.array(out["assign"]), in_caller, slow_quantile=args.slow_quantile)
+    t5 = time.perf_counter()
+    cpt = solver.critical_paths(hb, truth_all, in_caller, slow_quantile=args.slow_quantile)
+    names = [s.name for s in ok]
+    ep_names = [f"{s.name} -> callee {e}" for s in ok for e in range(s.problem.E)]
+    print(f"critical paths ({1e3 * (t5 - t4):.2f} ms): {int(cp['requests'][0])} requests, "
+          f"{int(cp['requests'][1])} slow (latency >= {cp['slow_us']:.1f} us, quantile {args.slow_quantile})")
+    share = lambda r, col: np.concatenate([r["server_us"][:, col], r["call_us"][:, col]]) / \
+        max(r["server_us"][:, col].sum() + r["call_us"][:, col].sum(), 1e-300)
+    rows = names + ep_names
+    pred = np.stack([share(cp, 0), share(cp, 1)], axis=1)
+    true = np.stack([share(cpt, 0), share(cpt, 1)], axis=1)
+    print(f"  {'service / callee edge':40s} {'all: pred':>10s} {'truth':>8s} {'slow: pred':>11s} {'truth':>8s}")
+    for k, name in enumerate(rows):
+        print(f"  {name:40s} {100 * pred[k, 0]:9.2f}% {100 * true[k, 0]:7.2f}% {100 * pred[k, 1]:10.2f}% "
+              f"{100 * true[k, 1]:7.2f}%")
+    diff = np.abs(pred - true)
+    k, col = np.unravel_index(int(np.argmax(diff)), diff.shape)
+    print(f"  largest difference: {100 * diff[k, col]:.2f} points at {rows[k]} ({('all', 'slow')[col]} requests)")
+    n_in = int(hb.prob_in_off[-1])
+    req = cp["request"]
+    slow_req = req[cp["latency_us"] >= cp["slow_us"]]
+    cul = cp["culprit"][slow_req]
+    in_prob = np.repeat(np.arange(len(ok)), np.diff(hb.prob_in_off))
+    out_ep = np.repeat(np.arange(len(ep_names)), np.diff(hb.ep_out_off))
+    owner = [names[in_prob[c]] if c < n_in else ep_names[out_ep[c - n_in]] for c in cul]
+    print("  culprits of the slow requests:")
+    for name, cnt in sorted(zip(*np.unique(owner, return_counts=True)), key=lambda t: -t[1]) if owner else []:
+        print(f"    {name:40s} {int(cnt):8d}")
+    ex = solver.assemble(hb, np.array(out["assign"]), in_caller, truth=truth_all)["exact"][req]
+    edges = np.quantile(cp["latency_us"], np.linspace(0, 1, 11))
+    dec = np.clip(np.searchsorted(edges, cp["latency_us"], side="right") - 1, 0, 9)
+    print("  exact requests per latency decile: " + " ".join(
+        f"{100 * (ex[dec == q] == 1).mean():.1f}%" if (dec == q).any() else "-" for q in range(10)))
 if args.traces:
     from traceweaver_b200 import traces
     in_caller = traces.caller_links(ok, hb)
@@ -78,7 +125,8 @@ if args.traces:
     t5 = time.perf_counter()
     ids = [i for s in ok for i in s.in_ids] + [i for s in ok for ids in s.out_ids for i in ids]
     np.savez(args.traces, parent=tr["parent"], root=tr["root"], size=tr["size"], exact=tr["exact"],
-             node_trace_id=np.array([t for t, _ in ids]), node_span_id=np.array([sid for _, sid in ids]))
+             node_trace_id=np.array([t for t, _ in ids]), node_span_id=np.array([sid for _, sid in ids]),
+             **({k: cp[k] for k in ("on_path", "self_us", "culprit")} if cp is not None else {}))
     n_in = int(hb.prob_in_off[-1])
     requests = int((tr["exact"] >= 0).sum())
     e2e = end_to_end_accuracy([[t for t, _ in s.in_ids] for s in ok], [s.truth for s in ok],

@@ -4,7 +4,7 @@ Field order and widths must match the header exactly; tests/test_abi.py checks s
 against values compiled from the header."""
 import ctypes as C
 
-TW_ABI_VERSION = 7
+TW_ABI_VERSION = 8
 TW_SCORE_KEEP_WINDOWS = 1
 TW_MAX_E = 8
 TW_K = 5
@@ -73,6 +73,11 @@ class TwSkipDesc(C.Structure):
 
 class TwSkipOut(C.Structure):
     _fields_ = [("pass_", TwPassOut), ("top2_score", P), ("top2_idx", P), ("top2_cnt", P), ("cut", P)]
+
+
+class TwCriticalOut(C.Structure):
+    _fields_ = [("root", P), ("on_path", P), ("self_us", P), ("culprit", P), ("server_us", P),
+                ("server_visits", P), ("call_us", P), ("requests", P)]
 
 
 class TwTraceKeys(C.Structure):

@@ -55,6 +55,9 @@ SYMBOLS = {
                                         C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tw_assemble_traces": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch), C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tw_critical_paths": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch),
+                                    C.POINTER(_abi.TwTimesF64), C.c_void_p, C.c_void_p, C.c_double,
+                                    C.POINTER(_abi.TwCriticalOut), C.c_void_p]),
 }
 
 

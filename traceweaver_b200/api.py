@@ -261,3 +261,23 @@ class BatchSolver:
             ref = traces.assemble(eng, hb, truth, links)
             out["exact"] = traces.exact_requests(res["root"], ref["root"], int(hb.prob_in_off[-1])).cpu().numpy()
         return out
+
+    def critical_paths(self, hb: HostBatch, assign, in_caller, slow_quantile=0.99):
+        """Where the time of every reconstructed request of `hb` went (tw_critical_paths; definition in
+        traces.py): `assign` in the layout of out["assign"], `in_caller` from traces.caller_links.  The slow
+        requests are those whose latency is at least the lower `slow_quantile`-quantile of all request
+        latencies (an actual latency, computed on the device).  Host arrays: root, on_path, self_us [nodes],
+        culprit [n_in], server_us / server_visits [P, 2] and call_us [n_ep, 2] (column 0 all requests,
+        column 1 slow ones), requests [2]; request (node ids of the request roots) and latency_us [requests];
+        slow_us, the threshold."""
+        from . import traces
+        eng = self.engine
+        spans = traces.upload_spans(eng, hb)
+        links = _to_device(dict(in_caller=np.asarray(in_caller, np.int32).reshape(-1)), eng.device)["in_caller"]
+        req, lat = traces.request_latencies(spans, links)
+        slow_us = traces.lower_quantile(lat, slow_quantile)
+        res = traces.critical_paths(eng, hb, assign, links, slow_us, spans=spans)
+        eng.status()                                      # a tree deeper than the walk can follow
+        out = {k: v.cpu().numpy() for k, v in res.items()}
+        out.update(request=req.cpu().numpy(), latency_us=lat.cpu().numpy(), slow_us=slow_us)
+        return out

@@ -101,7 +101,18 @@ struct tw_engine {
   // last call did (tw_debug_trace_rounds)
   DevBuf<int32_t> trace_claim;
   DevBuf<int32_t> trace_flags;
-  int trace_rounds_launched = 0, trace_rounds_run = 0;
+  int trace_rounds_launched = 0, trace_rounds_run = 0, trace_still = 0;
+  // critical paths (tw_critical_paths): the join's parent and size words, the walk's scratch (CpScratch),
+  // and the level launches of the last call (tw_debug_critical_levels)
+  DevBuf<int32_t> cp_parent;
+  DevBuf<int32_t> cp_size;
+  DevBuf<int32_t> cp_level;
+  DevBuf<int64_t> cp_wlo;
+  DevBuf<int64_t> cp_whi;
+  DevBuf<uint8_t> cp_slow;
+  DevBuf<unsigned long long> cp_cmax;
+  DevBuf<int> cp_act;
+  int cp_levels = 0;
   // skip / cache mode scratch (tw_skip_solve)
   DevBuf<uint32_t> skip_sets;
   DevBuf<int64_t> skip_set_off;
@@ -696,19 +707,23 @@ int tw_accuracy(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const in
   return TW_OK;
 }
 
-int tw_assemble_traces(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const int32_t* assign,
-                       const int32_t* in_caller, int32_t* parent_out, int32_t* root_out, int32_t* size_out,
-                       void* stream_) {
-  if (!eng || !dev || !assign || !in_caller || !parent_out || !root_out || !size_out)
-    return fail(TW_ERR_INVALID, "tw_assemble_traces: NULL argument");
-  int rc = validate_host(h, "tw_assemble_traces", false, true);
+// The host checks of tw_assemble_traces: the offset tables and int32 node ids.
+static int trace_check(const tw_batch* h, const char* who) {
+  int rc = validate_host(h, who, false, true);
   if (rc) return rc;
-  const int64_t n_in = h->n_in_total, n_out = h->n_out_total, n_nodes = n_in + n_out;
+  const int64_t n_nodes = h->n_in_total + h->n_out_total;
   if (n_nodes >= ((int64_t)1 << 31))
-    return fail(TW_ERR_RANGE_LIMIT, "tw_assemble_traces: %s nodes do not fit int32 node ids",
+    return fail(TW_ERR_RANGE_LIMIT, (std::string(who) + ": %s nodes do not fit int32 node ids").c_str(),
                 std::to_string(n_nodes).c_str());
-  cudaStream_t s = (cudaStream_t)stream_;
-  CU(cudaSetDevice(eng->device));
+  return TW_OK;
+}
+
+// The join of tw_assemble_traces after trace_check: its launches, the read-back of its error words and
+// round flags, and its errors (named after `who`).  Leaves the caller-claim words in eng->trace_claim.
+static int trace_join(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const int32_t* assign,
+                      const int32_t* in_caller, int32_t* parent_out, int32_t* root_out, int32_t* size_out,
+                      const char* who, cudaStream_t s) {
+  const int64_t n_in = h->n_in_total, n_out = h->n_out_total, n_nodes = n_in + n_out;
   const int rounds = trace_rounds(n_nodes);
   CU(eng->trace_claim.reserve((size_t)n_out));
   CU(eng->trace_flags.reserve((size_t)(4 + rounds)));
@@ -722,6 +737,8 @@ int tw_assemble_traces(tw_engine* eng, const tw_batch* dev, const tw_batch* h, c
   eng->trace_rounds_launched = rounds;
   eng->trace_rounds_run = 1;                               // round r > 0 runs iff round r - 1 moved a node
   while (eng->trace_rounds_run < rounds && flags[4 + eng->trace_rounds_run - 1]) ++eng->trace_rounds_run;
+  eng->trace_still = 0;                                    // the first round that moved no node (rounds: none)
+  while (eng->trace_still < rounds && flags[4 + eng->trace_still]) ++eng->trace_still;
   const int32_t none = 0x7f7f7f7f;
   const char* what[4] = {"out-span node %s is the child of two in-spans%s",
                          "out-span node %s is the caller of two in-spans%s",
@@ -729,9 +746,67 @@ int tw_assemble_traces(tw_engine* eng, const tw_batch* dev, const tw_batch* h, c
                          "in-span node %s has a caller that is not an out-span node%s"};
   for (int k : {3, 1, 2, 0})                               // the callers first, as traces.parents_host
     if (flags[k] != none) {
-      const std::string msg = std::string("tw_assemble_traces: ") + what[k];
+      const std::string msg = std::string(who) + ": " + what[k];
       return fail(TW_ERR_INVALID, msg.c_str(), std::to_string(flags[k]).c_str(), "");
     }
+  return TW_OK;
+}
+
+int tw_assemble_traces(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const int32_t* assign,
+                       const int32_t* in_caller, int32_t* parent_out, int32_t* root_out, int32_t* size_out,
+                       void* stream_) {
+  if (!eng || !dev || !assign || !in_caller || !parent_out || !root_out || !size_out)
+    return fail(TW_ERR_INVALID, "tw_assemble_traces: NULL argument");
+  int rc = trace_check(h, "tw_assemble_traces");
+  if (rc) return rc;
+  CU(cudaSetDevice(eng->device));
+  return trace_join(eng, dev, h, assign, in_caller, parent_out, root_out, size_out, "tw_assemble_traces",
+                    (cudaStream_t)stream_);
+}
+
+int tw_critical_paths(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const tw_times_f64* f64,
+                      const int32_t* assign, const int32_t* in_caller, double slow_us, const tw_critical_out* out,
+                      void* stream_) {
+  if (!eng || !dev || !assign || !in_caller || !out || !out->root || !out->on_path || !out->self_us ||
+      !out->culprit || !out->server_us || !out->server_visits || !out->call_us || !out->requests ||
+      (f64 ? (!f64->in_start || !f64->in_end || !f64->out_start || !f64->out_end)
+           : (!dev->in_start || !dev->in_end || !dev->out_start || !dev->out_end)))
+    return fail(TW_ERR_INVALID, "tw_critical_paths: NULL argument");
+  int rc = trace_check(h, "tw_critical_paths");
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream_;
+  CU(cudaSetDevice(eng->device));
+  const int64_t n_in = h->n_in_total, n_nodes = n_in + h->n_out_total;
+  CU(eng->cp_parent.reserve((size_t)n_nodes));
+  CU(eng->cp_size.reserve((size_t)n_nodes));
+  CU(eng->cp_level.reserve((size_t)n_in));
+  CU(eng->cp_wlo.reserve((size_t)n_in));
+  CU(eng->cp_whi.reserve((size_t)n_in));
+  CU(eng->cp_slow.reserve((size_t)n_in));
+  CU(eng->cp_cmax.reserve((size_t)n_in));
+  CU(eng->cp_act.reserve((size_t)kCpMaxLevels));
+  rc = trace_join(eng, dev, h, assign, in_caller, eng->cp_parent.p, out->root, eng->cp_size.p, "tw_critical_paths", s);
+  if (rc) return rc;
+  // Depth of the trees from the rounds: when round k moved no node, every node had reached its root in
+  // rounds 0 .. k - 1, which climb 2^k links (none when k = 0); an in-span at depth 2m links is walked at
+  // level m.  When every round moved a node (a cycle of links can keep moving), or the bound exceeds
+  // kCpMaxLevels: kCpMaxLevels.  Rounds run in place, so a node can climb further than 2^k links in them;
+  // the last level therefore walks whatever lies deeper itself.
+  int levels = kCpMaxLevels;
+  const int k = eng->trace_still;
+  if (k < eng->trace_rounds_launched && (k == 0 ? 1 : ((int64_t)1 << k) / 2 + 1) < kCpMaxLevels)
+    levels = k == 0 ? 1 : (int)(((int64_t)1 << k) / 2 + 1);
+  eng->cp_levels = levels;
+  CpScratch sc{eng->cp_level.p, eng->cp_wlo.p, eng->cp_whi.p, eng->cp_slow.p, eng->cp_cmax.p, eng->cp_act.p};
+  CU(launch_critical_paths(*dev, f64, assign, eng->trace_claim.p, slow_us, *out, sc, levels, eng->n_sm,
+                           eng->err_flag.p, s, eng->launches));
+  return TW_OK;
+}
+
+// Test hook, not part of the ABI header: the level launches of the last tw_critical_paths.
+int tw_debug_critical_levels(tw_engine* eng, int* levels) {
+  if (!eng || !levels) return fail(TW_ERR_INVALID, "tw_debug_critical_levels: NULL argument");
+  *levels = eng->cp_levels;
   return TW_OK;
 }
 

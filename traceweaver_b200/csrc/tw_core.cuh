@@ -1411,4 +1411,66 @@ struct WindowCursor {
   }
 };
 
+// ---------------------------------------------------------------------------------------------
+// Critical paths of the reconstructed requests (tw_critical_paths, tw_critical_path.cu).  T is the
+// time type of the batch: int64_t microseconds, or double for a time-compressed batch.  The steps use
+// min, max, add and subtract only, in a fixed order, so the host reference (traces.critical_paths_host)
+// repeats every window and self time bit for bit.
+// ---------------------------------------------------------------------------------------------
+
+// An on-path in-span with window [a, b] and its children, one per callee position e < E (has[e]: the
+// assignment gave it one, with interval [cs[e], ce[e]]).  Each child is clipped to the window and is
+// eligible iff what is left is not empty.  From the cursor c = b backwards: among the unchosen eligible
+// children that start before c, the one with the largest min(end, c) (the lowest callee position on a
+// tie) goes on the path with window [start, min(end, c)]; the gap up to c is the in-span's own time, and
+// c moves to the child's start.  What is left before the last chosen child is the in-span's own time
+// too.  on[e], [wlo[e], whi[e]]: the chosen children and their windows.  Returns the self time.
+template <class T>
+TW_HD T cp_in_span_step(int E, const bool* has, const T* cs, const T* ce, T a, T b, bool* on, T* wlo, T* whi) {
+  T s[TW_MAX_E], en[TW_MAX_E];
+  for (int e = 0; e < E; ++e) {
+    on[e] = false;
+    s[e] = cs[e] > a ? cs[e] : a;
+    en[e] = ce[e] < b ? ce[e] : b;
+  }
+  T c = b, self = 0;
+  for (;;) {
+    int best = -1;
+    T best_end = 0;
+    for (int e = 0; e < E; ++e) {
+      if (!has[e] || on[e] || !(en[e] > s[e]) || !(s[e] < c)) continue;
+      const T m = en[e] < c ? en[e] : c;
+      if (best < 0 || m > best_end) {
+        best = e;
+        best_end = m;
+      }
+    }
+    if (best < 0) break;
+    on[best] = true;
+    wlo[best] = s[best];
+    whi[best] = best_end;
+    self = self + (c - best_end);
+    c = s[best];
+  }
+  return self + (c - a);
+}
+
+// An on-path out-span with window [a, b] and its child in-span (has: the in-span that names it as its
+// caller, interval [ys, ye]).  The child is on the path iff its interval clipped to the window is not
+// empty (*on, window [*wlo, *whi]).  Returns the out-span's self time: the window less the child's.
+template <class T>
+TW_HD T cp_out_span_step(T a, T b, bool has, T ys, T ye, bool* on, T* wlo, T* whi) {
+  *on = false;
+  if (has) {
+    const T lo = ys > a ? ys : a, hi = ye < b ? ye : b;
+    if (hi > lo) {
+      *on = true;
+      *wlo = lo;
+      *whi = hi;
+      return (b - a) - (hi - lo);
+    }
+  }
+  return b - a;
+}
+
 }  // namespace tw

@@ -261,4 +261,22 @@ cudaError_t launch_assemble_traces(const tw_batch& b, int64_t n_tuple, const int
                                    int32_t* parent, int32_t* root, int32_t* size, int32_t* claim, int32_t* err,
                                    int* changed, int rounds, int n_sm, cudaStream_t s, int64_t& launches);
 
+// tw_critical_path.cu: the walk after the join.  Scratch per in-span: level (the level that walks it,
+// -1 = none yet), window (the time type's bits), slow (its request is slow; roots only), cmax (largest
+// self-time bits of the request; roots only); act: [levels] flags, level L put some in-span on the path.
+// claim: the join's caller-claim words (out-span -> the in-span that names it, -1).
+constexpr int kCpMaxLevels = 64;
+struct CpScratch {
+  int32_t* level;
+  int64_t* wlo;
+  int64_t* whi;
+  uint8_t* slow;
+  unsigned long long* cmax;
+  int* act;
+};
+cudaError_t launch_critical_paths(const tw_batch& b, const tw_times_f64* f64, const int32_t* assign,
+                                  const int32_t* claim, double slow_us, const tw_critical_out& out,
+                                  const CpScratch& sc, int levels, int n_sm, int* err_flag, cudaStream_t s,
+                                  int64_t& launches);
+
 }  // namespace tw
