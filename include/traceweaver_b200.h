@@ -480,8 +480,8 @@ int tw_assemble_traces(tw_engine* eng, const tw_batch* dev, const tw_batch* host
  * TW_ERR_INVALID / TW_ERR_RANGE_LIMIT errors of tw_assemble_traces, which it reads back); then one launch
  * per level of in-spans, as many as the join's pointer-jumping rounds allow for the depth of the trees
  * (at most 64), two culprit launches and one reduction.  In-spans deeper than the last level are walked by
- * its threads one after another; a tree too deep even for that sets TW_ERR_RANGE_LIMIT in the engine's
- * device status (tw_engine_status).  A bound batch is not touched.
+ * its threads one after another, without a stack: trees of any depth are walked, and every output is the
+ * same whatever the number of levels launched.  A bound batch is not touched.
  * ---------------------------------------------------------------------------------------------- */
 typedef struct tw_critical_out {
   int32_t* root;

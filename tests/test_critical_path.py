@@ -33,8 +33,9 @@ def emul(tmp_path_factory):
     return C.CDLL(so)
 
 
-def emul_paths(lib, hb, assign, in_caller, root, slow_us):
-    """The walk with the kernels' per-node steps, stepped on the CPU; the join's roots come in."""
+def emul_paths(lib, hb, assign, in_caller, root, slow_us, levels=0):
+    """The walk with the kernels' per-node steps, stepped on the CPU; the join's roots come in.  levels: the
+    level launches, the last of them walking what lies below it (cp_tail_walk); 0: until nothing is left."""
     a = {k: np.ascontiguousarray(v) for k, v in hb.arrays.items()}
     st = batch_struct(HostBatch(problems=hb.problems, arrays=a), lambda k: a[k].ctypes.data)
     times = _abi.fill(_abi.TwTimesF64, a) if hb.float_times else None
@@ -46,7 +47,7 @@ def emul_paths(lib, hb, assign, in_caller, root, slow_us):
     links = [np.ascontiguousarray(x, np.int32).reshape(-1) for x in (assign, in_caller, root)]
     ptr = lambda x: C.c_void_p(x.ctypes.data)
     rc = lib.twe_critical_paths(C.byref(st), C.byref(times) if times is not None else None,
-                                *[ptr(x) for x in links], C.c_double(slow_us),
+                                *[ptr(x) for x in links], C.c_double(slow_us), C.c_int(levels),
                                 *[ptr(out[k]) for k in ("on_path", "self_us", "culprit", "server_us", "server_visits",
                                                         "call_us", "requests")])
     assert rc == 0

@@ -277,7 +277,7 @@ class BatchSolver:
         req, lat = traces.request_latencies(spans, links)
         slow_us = traces.lower_quantile(lat, slow_quantile)
         res = traces.critical_paths(eng, hb, assign, links, slow_us, spans=spans)
-        eng.status()                                      # a tree deeper than the walk can follow
+        eng.status()                                      # syncs the stream, raises on engine errors
         out = {k: v.cpu().numpy() for k, v in res.items()}
         out.update(request=req.cpu().numpy(), latency_us=lat.cpu().numpy(), slow_us=slow_us)
         return out

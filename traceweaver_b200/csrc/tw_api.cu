@@ -103,7 +103,8 @@ struct tw_engine {
   DevBuf<int32_t> trace_flags;
   int trace_rounds_launched = 0, trace_rounds_run = 0, trace_still = 0;
   // critical paths (tw_critical_paths): the join's parent and size words, the walk's scratch (CpScratch),
-  // and the level launches of the last call (tw_debug_critical_levels)
+  // the level launches of the last call (tw_debug_critical_levels) and a forced level count, 0 = from the
+  // rounds (tw_debug_critical_force_levels)
   DevBuf<int32_t> cp_parent;
   DevBuf<int32_t> cp_size;
   DevBuf<int32_t> cp_level;
@@ -112,7 +113,7 @@ struct tw_engine {
   DevBuf<uint8_t> cp_slow;
   DevBuf<unsigned long long> cp_cmax;
   DevBuf<int> cp_act;
-  int cp_levels = 0;
+  int cp_levels = 0, cp_force_levels = 0;
   // skip / cache mode scratch (tw_skip_solve)
   DevBuf<uint32_t> skip_sets;
   DevBuf<int64_t> skip_set_off;
@@ -790,16 +791,28 @@ int tw_critical_paths(tw_engine* eng, const tw_batch* dev, const tw_batch* h, co
   // Depth of the trees from the rounds: when round k moved no node, every node had reached its root in
   // rounds 0 .. k - 1, which climb 2^k links (none when k = 0); an in-span at depth 2m links is walked at
   // level m.  When every round moved a node (a cycle of links can keep moving), or the bound exceeds
-  // kCpMaxLevels: kCpMaxLevels.  Rounds run in place, so a node can climb further than 2^k links in them;
-  // the last level therefore walks whatever lies deeper itself.
+  // kCpMaxLevels: kCpMaxLevels.  Rounds run in place, so a node can climb further than 2^k links in them
+  // and the count depends on the order threads ran in; the last level walks whatever lies deeper itself,
+  // so only the launch count does, not the results.
   int levels = kCpMaxLevels;
   const int k = eng->trace_still;
   if (k < eng->trace_rounds_launched && (k == 0 ? 1 : ((int64_t)1 << k) / 2 + 1) < kCpMaxLevels)
     levels = k == 0 ? 1 : (int)(((int64_t)1 << k) / 2 + 1);
+  if (eng->cp_force_levels) levels = eng->cp_force_levels;
   eng->cp_levels = levels;
   CpScratch sc{eng->cp_level.p, eng->cp_wlo.p, eng->cp_whi.p, eng->cp_slow.p, eng->cp_cmax.p, eng->cp_act.p};
-  CU(launch_critical_paths(*dev, f64, assign, eng->trace_claim.p, slow_us, *out, sc, levels, eng->n_sm,
-                           eng->err_flag.p, s, eng->launches));
+  CU(launch_critical_paths(*dev, f64, assign, eng->trace_claim.p, eng->cp_parent.p, slow_us, *out, sc, levels,
+                           eng->n_sm, s, eng->launches));
+  return TW_OK;
+}
+
+// Test hook, not part of the ABI header: later tw_critical_paths calls launch `levels` levels (1 ..
+// kCpMaxLevels), or as many as the join's rounds give (0).
+int tw_debug_critical_force_levels(tw_engine* eng, int levels) {
+  if (!eng) return fail(TW_ERR_INVALID, "tw_debug_critical_force_levels: NULL engine");
+  if (levels < 0 || levels > kCpMaxLevels)
+    return fail(TW_ERR_INVALID, "tw_debug_critical_force_levels: %s levels (0 .. 64)", std::to_string(levels).c_str());
+  eng->cp_force_levels = levels;
   return TW_OK;
 }
 

@@ -1473,4 +1473,35 @@ TW_HD T cp_out_span_step(T a, T b, bool has, T ys, T ye, bool* on, T* wlo, T* wh
   return b - a;
 }
 
+// The last level's walk of everything on the path below in-span x, which it has just visited: depth
+// first, without a stack, so any depth is walked.  `g` gives the tree:
+//   g.enter(y)    y's callee count; g.child then looks at y's callees
+//   g.child(e)    the in-span at callee position e of the entered in-span if the entered in-span's visit
+//                 put it on the path (marked it), else -1
+//   g.visit(y)    walks in-span y (its window is set): the per-node steps, and marks the in-spans it puts
+//                 on the path
+//   g.up(y, &e)   y's parent in-span, and y's callee position in it
+// The walk goes down to the first marked child in callee order; from an in-span with no marked child
+// after position e it climbs to the parent and looks on after its own position, so every marked in-span
+// is visited once.  It ends back at x.  No result depends on the order: a visit reads only its own window.
+template <class G>
+TW_HD void cp_tail_walk(G& g, int32_t x) {
+  int32_t y = x;
+  int e = 0;
+  for (;;) {
+    const int E = g.enter(y);
+    int32_t c = -1;
+    while (e < E && (c = g.child(e)) < 0) ++e;
+    if (c >= 0) {
+      g.visit(c);
+      y = c;
+      e = 0;
+      continue;
+    }
+    if (y == x) return;
+    y = g.up(y, &e);
+    ++e;
+  }
+}
+
 }  // namespace tw

@@ -3,10 +3,12 @@
 // After the join (tw_traces.cu) every request is a tree of nodes.  Windows are handed down the trees one
 // level of in-spans per launch: a thread takes an on-path in-span, chooses which of its out-spans are on
 // the path (cp_in_span_step, tw_core.cuh), and for each of them whether the callee's in-span is
-// (cp_out_span_step), whose window it writes for the next level.  Then every request's culprit, by an
-// integer max over the bits of the (non-negative) self times and a min over the node ids that hold it,
-// and the per-service sums, one CTA per service or callee in a fixed order.  No float atomics: every
-// result is the same from run to run and for any grid.
+// (cp_out_span_step), whose window it writes for the next level.  The last level walks everything below
+// its in-spans itself, without a stack (cp_tail_walk), so no result depends on how many levels were
+// launched.  Then every request's culprit, by an integer max over the bits of the (non-negative) self
+// times and a min over the node ids that hold it, and the per-service sums, one CTA per service or callee
+// in a fixed order.  No float atomics: every result is the same from run to run, for any grid and any
+// level count.
 #include "tw_kernels.cuh"
 
 namespace tw {
@@ -14,7 +16,6 @@ namespace tw {
 namespace {
 
 constexpr int kCpThreads = 256;
-constexpr int kCpTailStack = 64;                 // in-spans a thread of the last level keeps pending
 
 template <class T>
 struct CpTimes {
@@ -34,11 +35,12 @@ __device__ __forceinline__ int cp_last_le(const int64_t* off, int n, int64_t key
 }
 
 // In-span x on the path with window [a, b]: its self time, its chosen out-spans' self times, and the
-// windows of the callee in-spans that go on the path, whose ids land in next[] (returns their count).
+// windows of the callee in-spans that go on the path, whose level words become `mark` (returns their
+// count).
 template <class T>
 __device__ int cp_visit(const tw_batch& bt, const CpTimes<T>& t, const int32_t* __restrict__ assign,
-                        const int32_t* __restrict__ claim, const tw_critical_out& out, T* wlo, T* whi, int32_t x,
-                        T a, T b, int32_t* next) {
+                        const int32_t* __restrict__ claim, const tw_critical_out& out, T* wlo, T* whi,
+                        int32_t* level, int32_t x, T a, T b, int mark) {
   const int32_t n_in = (int32_t)bt.n_in_total;
   const int p = cp_last_le(bt.prob_in_off, bt.n_problems, x);
   const int64_t in0 = bt.prob_in_off[p], n = bt.prob_in_off[p + 1] - in0, i = x - in0;
@@ -69,21 +71,66 @@ __device__ int cp_visit(const tw_batch& bt, const CpTimes<T>& t, const int32_t* 
     if (y_on) {
       wlo[y] = ylo;
       whi[y] = yhi;
-      next[m++] = y;
+      level[y] = mark;
+      ++m;
     }
   }
   return m;
 }
 
+// The trees below the last level L for cp_tail_walk (tw_core.cuh): children through `assign` and the
+// caller-claim words, marked when their level word is L + 1; parents through the join's parent words.
+template <class T>
+struct CpTail {
+  const tw_batch& bt;
+  const CpTimes<T>& t;
+  const int32_t* __restrict__ assign;
+  const int32_t* __restrict__ claim;
+  const int32_t* __restrict__ parent;
+  const tw_critical_out& out;
+  const CpScratch& sc;
+  int mark;
+  int64_t tup, n, i;                             // the entered in-span: its service's tuples, size, own index
+  int ep0;                                       // and the service's first global callee
+
+  __device__ int enter(int32_t y) {
+    const int p = cp_last_le(bt.prob_in_off, bt.n_problems, y);
+    const int64_t in0 = bt.prob_in_off[p];
+    tup = bt.prob_tuple_off[p];
+    n = bt.prob_in_off[p + 1] - in0;
+    i = y - in0;
+    ep0 = bt.prob_ep_off[p];
+    return bt.prob_ep_off[p + 1] - ep0;
+  }
+  __device__ int32_t child(int e) const {
+    const int32_t j = assign[tup + e * n + i];
+    if (j < 0) return -1;
+    const int32_t y = claim[bt.ep_out_off[ep0 + e] + j];
+    return y >= 0 && sc.level[y] == mark ? y : -1;
+  }
+  __device__ void visit(int32_t y) {
+    T* wlo = (T*)sc.wlo;
+    T* whi = (T*)sc.whi;
+    cp_visit<T>(bt, t, assign, claim, out, wlo, whi, sc.level, y, wlo[y], whi[y], mark);
+  }
+  __device__ int32_t up(int32_t y, int* e) const {
+    const int32_t k = parent[y];                 // y's caller: out-span node n_in + its index
+    const int32_t x = parent[k];
+    const int ep = cp_last_le(bt.ep_out_off, bt.n_ep_total, (int64_t)k - bt.n_in_total);
+    *e = ep - bt.prob_ep_off[cp_last_le(bt.prob_in_off, bt.n_problems, x)];
+    return x;
+  }
+};
+
 // Level L: one thread per in-span walked at L (level 0: the request roots, whose windows are their own
 // intervals).  The in-spans it puts on the path are walked at L + 1.  A level after one that put nothing
-// on the path returns at once.  The last level (`last`) walks what it puts on the path itself, depth first.
-// Level 0 also sets culprit[] to INT_MAX for a root and -1 otherwise, flags the slow requests and counts
-// the requests.
+// on the path returns at once.  The last level (`last`) walks what lies below its in-spans itself
+// (cp_tail_walk), at any depth.  Level 0 also sets culprit[] to INT_MAX for a root and -1 otherwise, flags
+// the slow requests and counts the requests.
 template <class T>
 __global__ void __launch_bounds__(kCpThreads)
 k_cp_level(tw_batch bt, CpTimes<T> t, const int32_t* __restrict__ assign, const int32_t* __restrict__ claim,
-           tw_critical_out out, CpScratch sc, int L, int last, double slow_us, int* __restrict__ err_flag) {
+           const int32_t* __restrict__ parent, tw_critical_out out, CpScratch sc, int L, int last, double slow_us) {
   if (L > 0 && *(volatile int*)&sc.act[L - 1] == 0) return;
   const int64_t n_in = bt.n_in_total;
   T* wlo = (T*)sc.wlo;
@@ -109,26 +156,11 @@ k_cp_level(tw_batch bt, CpTimes<T> t, const int32_t* __restrict__ assign, const 
       a = wlo[x];
       b = whi[x];
     }
-    int32_t next[TW_MAX_E];
-    const int m = cp_visit<T>(bt, t, assign, claim, out, wlo, whi, x, a, b, next);
+    const int m = cp_visit<T>(bt, t, assign, claim, out, wlo, whi, sc.level, x, a, b, L + 1);
     activated |= m > 0;
-    if (!last) {
-      for (int q = 0; q < m; ++q) sc.level[next[q]] = L + 1;
-      continue;
-    }
-    int32_t stack[kCpTailStack];
-    int sp = 0;
-    for (int q = 0; q < m; ++q) {
-      if (sp < kCpTailStack) stack[sp++] = next[q];
-      else atomicMin(err_flag, (int)TW_ERR_RANGE_LIMIT);
-    }
-    while (sp > 0) {
-      const int32_t y = stack[--sp];
-      const int mm = cp_visit<T>(bt, t, assign, claim, out, wlo, whi, y, wlo[y], whi[y], next);
-      for (int q = 0; q < mm; ++q) {
-        if (sp < kCpTailStack) stack[sp++] = next[q];
-        else atomicMin(err_flag, (int)TW_ERR_RANGE_LIMIT);
-      }
+    if (last && m > 0) {
+      CpTail<T> g{bt, t, assign, claim, parent, out, sc, L + 1};
+      cp_tail_walk(g, x);
     }
   }
   if (__syncthreads_or(activated) && threadIdx.x == 0) sc.act[L] = 1;
@@ -235,11 +267,11 @@ unsigned cp_grid(int64_t n, int n_sm) {
 
 template <class T>
 cudaError_t launch_walk(const tw_batch& b, const CpTimes<T>& t, const int32_t* assign, const int32_t* claim,
-                        double slow_us, const tw_critical_out& out, const CpScratch& sc, int levels, int n_sm,
-                        int* err_flag, cudaStream_t s, int64_t& launches) {
+                        const int32_t* parent, double slow_us, const tw_critical_out& out, const CpScratch& sc,
+                        int levels, int n_sm, cudaStream_t s, int64_t& launches) {
   const unsigned g = cp_grid(b.n_in_total, n_sm);
   for (int L = 0; L < levels; ++L) {
-    k_cp_level<T><<<g, kCpThreads, 0, s>>>(b, t, assign, claim, out, sc, L, L == levels - 1, slow_us, err_flag);
+    k_cp_level<T><<<g, kCpThreads, 0, s>>>(b, t, assign, claim, parent, out, sc, L, L == levels - 1, slow_us);
     const cudaError_t e = after_launch(launches);
     if (e != cudaSuccess) return e;
   }
@@ -249,9 +281,9 @@ cudaError_t launch_walk(const tw_batch& b, const CpTimes<T>& t, const int32_t* a
 }  // namespace
 
 cudaError_t launch_critical_paths(const tw_batch& b, const tw_times_f64* f64, const int32_t* assign,
-                                  const int32_t* claim, double slow_us, const tw_critical_out& out,
-                                  const CpScratch& sc, int levels, int n_sm, int* err_flag, cudaStream_t s,
-                                  int64_t& launches) {
+                                  const int32_t* claim, const int32_t* parent, double slow_us,
+                                  const tw_critical_out& out, const CpScratch& sc, int levels, int n_sm,
+                                  cudaStream_t s, int64_t& launches) {
   const int64_t n_in = b.n_in_total, n_nodes = n_in + b.n_out_total;
   cudaError_t e;
   if ((e = cudaMemsetAsync(out.on_path, 0, (size_t)n_nodes, s)) != cudaSuccess) return e;
@@ -262,10 +294,10 @@ cudaError_t launch_critical_paths(const tw_batch& b, const tw_times_f64* f64, co
   if ((e = cudaMemsetAsync(sc.act, 0, (size_t)levels * sizeof(int), s)) != cudaSuccess) return e;
   if (f64)
     e = launch_walk<double>(b, CpTimes<double>{f64->in_start, f64->in_end, f64->out_start, f64->out_end}, assign,
-                            claim, slow_us, out, sc, levels, n_sm, err_flag, s, launches);
+                            claim, parent, slow_us, out, sc, levels, n_sm, s, launches);
   else
     e = launch_walk<int64_t>(b, CpTimes<int64_t>{b.in_start, b.in_end, b.out_start, b.out_end}, assign, claim,
-                             slow_us, out, sc, levels, n_sm, err_flag, s, launches);
+                             parent, slow_us, out, sc, levels, n_sm, s, launches);
   if (e != cudaSuccess) return e;
   const unsigned g = cp_grid(n_nodes, n_sm);
   k_cp_culprit_max<<<g, kCpThreads, 0, s>>>(n_nodes, out.on_path, out.root, out.self_us, sc.cmax);

@@ -264,7 +264,8 @@ cudaError_t launch_assemble_traces(const tw_batch& b, int64_t n_tuple, const int
 // tw_critical_path.cu: the walk after the join.  Scratch per in-span: level (the level that walks it,
 // -1 = none yet), window (the time type's bits), slow (its request is slow; roots only), cmax (largest
 // self-time bits of the request; roots only); act: [levels] flags, level L put some in-span on the path.
-// claim: the join's caller-claim words (out-span -> the in-span that names it, -1).
+// claim: the join's caller-claim words (out-span -> the in-span that names it, -1); parent: the join's
+// parent words.  Any levels >= 1 gives the same results: the last level walks what lies below it.
 constexpr int kCpMaxLevels = 64;
 struct CpScratch {
   int32_t* level;
@@ -275,8 +276,8 @@ struct CpScratch {
   int* act;
 };
 cudaError_t launch_critical_paths(const tw_batch& b, const tw_times_f64* f64, const int32_t* assign,
-                                  const int32_t* claim, double slow_us, const tw_critical_out& out,
-                                  const CpScratch& sc, int levels, int n_sm, int* err_flag, cudaStream_t s,
-                                  int64_t& launches);
+                                  const int32_t* claim, const int32_t* parent, double slow_us,
+                                  const tw_critical_out& out, const CpScratch& sc, int levels, int n_sm,
+                                  cudaStream_t s, int64_t& launches);
 
 }  // namespace tw

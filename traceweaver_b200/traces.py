@@ -210,8 +210,8 @@ def critical_paths(engine, hb, assign, in_caller, slow_us, spans=None):
     touched).  assign, in_caller as for assemble; slow_us: requests with latency >= slow_us form the second
     column of the sums; spans: upload_spans(engine, hb) when the caller already has it.  Returns device
     tensors: root int32 [N], on_path uint8 [N], self_us float64 [N], culprit int32 [n_in], server_us float64
-    [P, 2], server_visits int32 [P, 2], call_us float64 [n_ep, 2], requests int32 [2].  A tree deeper than the
-    walk can follow shows in engine.status() (TW_ERR_RANGE_LIMIT)."""
+    [P, 2], server_visits int32 [P, 2], call_us float64 [n_ep, 2], requests int32 [2].  Trees of any depth
+    are walked, with the same results whatever the number of level launches."""
     dev = engine.device
     d = _to_device({k: hb.arrays[k] for k in _OFFSETS}, dev)
     d.update(spans if spans is not None else upload_spans(engine, hb))
