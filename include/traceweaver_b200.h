@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define TW_ABI_VERSION 8
+#define TW_ABI_VERSION 9
 
 /* Algorithm constants hard-coded by the reference. */
 #define TW_MAX_E 8             /* engine limit on out-eps per service (shipped data: <= 4)      */
@@ -496,6 +496,66 @@ typedef struct tw_critical_out {
 int tw_critical_paths(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc,
                       const tw_times_f64* dev_times_f64, const int32_t* assign, const int32_t* in_caller,
                       double slow_us, const tw_critical_out* out, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Confidence of the reconstructed requests, without a ground truth.  This project's own definition.  Nodes,
+ * links and requests are those of tw_assemble_traces; every in-span is one reconstruction decision.  Inputs
+ * per in-span x: its chosen tuple in `assign`, score[x] / code[x] of that tuple from tw_score_assignments
+ * (under the final parameters), and the final no-deletion top-K row of `final_topk` (tw_score_topk; only
+ * topk_score / topk_idx / topk_cnt are read), the list the margin is measured against.
+ *   choice probability p_x: the chosen tuple's share of the likelihood among the alternatives the engine
+ *     listed.  0 unless code[x] == TW_ASSESS_SCORED (NA, out of range, infeasible) or when score[x] is -inf.
+ *     Else, with A the listed ranks r < topk_cnt[x] whose tuple differs from the chosen one at some callee
+ *     position, s_c = score[x] and m = max(s_c, max_A s_r):
+ *       S = exp(s_c - m) + sum over r in A, ascending, of exp(s_r - m),   p_x = exp(s_c - m) / S.
+ *     A single candidate gives 1; a chosen tuple the list does not hold counts with its own score.  It
+ *     ignores the windows' conflicts and the tuples beyond rank K, so it is pessimistic; it is a ranking
+ *     signal, not a calibrated probability.
+ *   ell_x = -log p_x, formed as log(S) + (m - s_c); +inf where p_x == 0 (also when exp underflows).
+ * exp and log are the engine's own (conf_exp, conf_log in tw_core.cuh, within 2 ulp): the CPU build of the
+ * step and a NumPy restatement give the same bits.  Outputs, all DEVICE buffers of the caller
+ * (N = n_in_total + n_out_total):
+ *   root           int32 [N]       as tw_assemble_traces' root_out
+ *   p, ell         double [n_in]   per in-span
+ *   for an in-span root r (a request; in-spans on or under a cycle and in detached fragments belong to none):
+ *   decisions      int32 [n_in]    in-spans whose root is r (0 for a non-root)
+ *   zero           int32 [n_in]    of them, those with p == 0
+ *   log_conf       int64 [n_in]    sum of the others' ell, each rounded to a multiple of 2^-32 nats (nearest,
+ *                                  ties to even) and added as integers: exact and order-free
+ *   conf           double [n_in]   exp(-log_conf * 2^-32), 0 when zero[r] > 0; NaN for a non-root
+ *   weakest        int32 [n_in]    the in-span of the request with the smallest p (smallest node id on a
+ *                                  tie; an integer min over the bits of p); -1 for a non-root
+ *   weakest_p      double [n_in]   its p; NaN for a non-root
+ *   est_accuracy   double [P]      mean p over the service's in-spans: the truth-free counterpart of its
+ *                                  accuracy
+ *   requests       int32 [1]       number of requests
+ *   expected_exact double [1]      sum of conf over the requests: the truth-free counterpart of the number of
+ *                                  exactly reconstructed requests
+ * The float sums are fixed-order reductions (one CTA per service, then one CTA over the services): bit-
+ * identical from run to run and whatever grouping produced the inputs.  Limits: a finite ell is below 748, so
+ * a term is below 2^42 units and a request of fewer than 2^21 decisions cannot overflow log_conf; a larger
+ * one returns TW_ERR_RANGE_LIMIT naming it.  The join runs inside (limits and TW_ERR_INVALID /
+ * TW_ERR_RANGE_LIMIT errors of tw_assemble_traces, which it reads back), then four launches: the per-in-span
+ * step, the per-request pass, the per-service reduction and the batch total.  Span times are not read and a
+ * bound batch is not touched.  Blocks until `stream` is idle.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct tw_confidence_out {
+  int32_t* root;
+  double* p;
+  double* ell;
+  int32_t* decisions;
+  int32_t* zero;
+  int64_t* log_conf;
+  double* conf;
+  int32_t* weakest;
+  double* weakest_p;
+  double* est_accuracy;
+  int32_t* requests;
+  double* expected_exact;
+} tw_confidence_out;
+int tw_request_confidence(tw_engine* eng, const tw_batch* dev, const tw_batch* host_desc, const int32_t* assign,
+                          const int32_t* in_caller, const double* score, const uint8_t* code,
+                          const tw_score_out* final_topk, const tw_confidence_out* out, void* stream);
 
 #ifdef __cplusplus
 }

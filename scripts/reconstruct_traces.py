@@ -18,7 +18,13 @@ node_span_id; it prints the share of exact requests beside the end-to-end accura
 edge, the share of the requests' critical time spent there, over all requests and over the slow ones (latency at
 or above the --slow-quantile of all latencies), on the predicted assignment and on the truth, and the largest
 difference between the two; the services the slow requests' culprits belong to; and the share of exact requests
-per latency decile.  With --traces the file also holds on_path, self_us and culprit of the prediction."""
+per latency decile.  With --traces the file also holds on_path, self_us and culprit of the prediction.
+--confidence (BatchSolver.request_confidence; definition in traceweaver_b200/traces.py) prints, per service, the
+truth-free est_accuracy beside the measured accuracy and the share of in-spans the window's MWIS did not give
+their best tuple (not_best_count / n_in); the batch's expected_exact beside the exact share of requests; the
+requests by confidence bin against their exact flag; and with --critical-path the culprit services of the slow
+requests, split into confident (conf >= 0.99) and unconfident ones.  With --traces the file also holds conf,
+weakest and p."""
 import argparse, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -31,6 +37,7 @@ ap.add_argument("--seed", type=int, default=10)
 ap.add_argument("--likelihood", action="store_true", help="print per-service confidence and error classes")
 ap.add_argument("--traces", default=None, metavar="FILE.npz", help="write the reconstructed request trees")
 ap.add_argument("--critical-path", action="store_true", help="print where the requests' time went")
+ap.add_argument("--confidence", action="store_true", help="print how sure each reconstruction is, without the truth")
 ap.add_argument("--slow-quantile", type=float, default=0.99, help="latency quantile of the slow requests")
 args = ap.parse_args()
 
@@ -51,7 +58,8 @@ hb = to_host_batch(ok)
 solver = BatchSolver(device=args.device, seed_select=args.seed)
 solver.solve(hb)                                   # warm-up: allocations, random streams
 t2 = time.perf_counter()
-out = solver.solve(hb, want_likelihood=args.likelihood, want_mixtures=args.likelihood)
+out = solver.solve(hb, want_likelihood=args.likelihood or args.confidence, want_mixtures=args.likelihood,
+                   want_scores=args.confidence)
 t3 = time.perf_counter()
 n_spans = sum(s.problem.n_in * (1 + s.problem.E) for s in ok)
 print(f"solved {n_spans} spans in {1e3 * (t3 - t2):.2f} ms (host buffers in and out)")
@@ -116,6 +124,46 @@ if args.critical_path:
     dec = np.clip(np.searchsorted(edges, cp["latency_us"], side="right") - 1, 0, 9)
     print("  exact requests per latency decile: " + " ".join(
         f"{100 * (ex[dec == q] == 1).mean():.1f}%" if (dec == q).any() else "-" for q in range(10)))
+cf = None
+if args.confidence:
+    from traceweaver_b200 import traces
+    in_caller = traces.caller_links(ok, hb)
+    truth_all = np.concatenate([s.truth.reshape(-1) for s in ok]).astype(np.int32)
+    t4 = time.perf_counter()
+    cf = solver.request_confidence(hb, out, in_caller)
+    t5 = time.perf_counter()
+    print(f"request confidence ({1e3 * (t5 - t4):.2f} ms): {cf['requests']} requests")
+    print(f"  {'service':28s} {'accuracy':>9s} {'est_accuracy':>13s} {'not_best/n_in':>14s}")
+    for p, s in enumerate(ok):
+        a = out["assign"][int(hb.prob_tuple_off[p]):int(hb.prob_tuple_off[p + 1])]
+        print(f"  {s.name:28s} {100 * accuracy(s, a):8.3f}% {100 * cf['est_accuracy'][p]:12.3f}% "
+              f"{100 * out['counters'][p, 0] / s.problem.n_in:13.3f}%")
+    req = cf["request"]
+    ex = solver.assemble(hb, np.array(out["assign"]), in_caller, truth=truth_all)["exact"][req] == 1
+    conf = cf["conf"][req]
+    print(f"  expected_exact {cf['expected_exact']:.1f} of {len(req)} requests ({100 * cf['expected_exact'] / max(len(req), 1):.3f} %)"
+          f"  exact {int(ex.sum())} ({100 * ex.mean() if len(req) else 0.0:.3f} %)")
+    edges = (0.0, 0.5, 0.8, 0.95, 0.99, 1.0)
+    print(f"  {'conf bin':16s} {'requests':>9s} {'exact':>8s} {'mean conf':>10s}")
+    for lo, hi in zip(edges[:-1], edges[1:]):
+        sel = (conf >= lo) & ((conf < hi) if hi < 1.0 else (conf <= hi))
+        if sel.any():
+            print(f"  [{lo:.2f}, {hi:.2f}{')' if hi < 1.0 else ']'}     {int(sel.sum()):9d} {100 * ex[sel].mean():7.2f}% "
+                  f"{100 * conf[sel].mean():9.2f}%")
+    if cp is not None:
+        n_in = int(hb.prob_in_off[-1])
+        names = [s.name for s in ok]
+        ep_names = [f"{s.name} -> callee {e}" for s in ok for e in range(s.problem.E)]
+        in_prob = np.repeat(np.arange(len(ok)), np.diff(hb.prob_in_off))
+        out_ep = np.repeat(np.arange(len(ep_names)), np.diff(hb.ep_out_off))
+        slow_req = cp["request"][cp["latency_us"] >= cp["slow_us"]]
+        for label, sel in (("confident (conf >= 0.99)", cf["conf"][slow_req] >= 0.99),
+                           ("unconfident (conf < 0.99)", cf["conf"][slow_req] < 0.99)):
+            cul = cp["culprit"][slow_req[sel]]
+            owner = [names[in_prob[c]] if c < n_in else ep_names[out_ep[c - n_in]] for c in cul]
+            print(f"  culprits of the slow requests, {label}: {int(sel.sum())}")
+            for name, cnt in sorted(zip(*np.unique(owner, return_counts=True)), key=lambda t: -t[1]) if owner else []:
+                print(f"    {name:40s} {int(cnt):8d}")
 if args.traces:
     from traceweaver_b200 import traces
     in_caller = traces.caller_links(ok, hb)
@@ -126,7 +174,8 @@ if args.traces:
     ids = [i for s in ok for i in s.in_ids] + [i for s in ok for ids in s.out_ids for i in ids]
     np.savez(args.traces, parent=tr["parent"], root=tr["root"], size=tr["size"], exact=tr["exact"],
              node_trace_id=np.array([t for t, _ in ids]), node_span_id=np.array([sid for _, sid in ids]),
-             **({k: cp[k] for k in ("on_path", "self_us", "culprit")} if cp is not None else {}))
+             **({k: cp[k] for k in ("on_path", "self_us", "culprit")} if cp is not None else {}),
+             **({k: cf[k] for k in ("conf", "weakest", "p")} if cf is not None else {}))
     n_in = int(hb.prob_in_off[-1])
     requests = int((tr["exact"] >= 0).sum())
     e2e = end_to_end_accuracy([[t for t, _ in s.in_ids] for s in ok], [s.truth for s in ok],

@@ -4,7 +4,7 @@ Field order and widths must match the header exactly; tests/test_abi.py checks s
 against values compiled from the header."""
 import ctypes as C
 
-TW_ABI_VERSION = 8
+TW_ABI_VERSION = 9
 TW_SCORE_KEEP_WINDOWS = 1
 TW_MAX_E = 8
 TW_K = 5
@@ -78,6 +78,11 @@ class TwSkipOut(C.Structure):
 class TwCriticalOut(C.Structure):
     _fields_ = [("root", P), ("on_path", P), ("self_us", P), ("culprit", P), ("server_us", P),
                 ("server_visits", P), ("call_us", P), ("requests", P)]
+
+
+class TwConfidenceOut(C.Structure):
+    _fields_ = [("root", P), ("p", P), ("ell", P), ("decisions", P), ("zero", P), ("log_conf", P), ("conf", P),
+                ("weakest", P), ("weakest_p", P), ("est_accuracy", P), ("requests", P), ("expected_exact", P)]
 
 
 class TwTraceKeys(C.Structure):

@@ -58,6 +58,9 @@ SYMBOLS = {
     "tw_critical_paths": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch),
                                     C.POINTER(_abi.TwTimesF64), C.c_void_p, C.c_void_p, C.c_double,
                                     C.POINTER(_abi.TwCriticalOut), C.c_void_p]),
+    "tw_request_confidence": (C.c_int, [C.c_void_p, C.POINTER(_abi.TwBatch), C.POINTER(_abi.TwBatch), C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(_abi.TwScoreOut),
+                                        C.POINTER(_abi.TwConfidenceOut), C.c_void_p]),
 }
 
 

@@ -281,3 +281,30 @@ class BatchSolver:
         out = {k: v.cpu().numpy() for k, v in res.items()}
         out.update(request=req.cpu().numpy(), latency_us=lat.cpu().numpy(), slow_us=slow_us)
         return out
+
+    def request_confidence(self, hb: HostBatch, out, in_caller):
+        """How sure the reconstruction of every request of `hb` is, without a ground truth
+        (tw_request_confidence; definition in traces.py).  `out`: a solve(hb, want_likelihood=True,
+        want_scores=True) result, or any dict with the same keys: assign, chosen_score, chosen_code (the chosen
+        tuples' scores, e.g. from score()), topk_score, topk_idx, topk_cnt (the final no-deletion top-K).
+        `in_caller` from traces.caller_links.  Host arrays: root [nodes]; p, ell, decisions, zero, log_conf
+        (int64, units of 2^-32 nats), conf, weakest, weakest_p [n_in]; est_accuracy [P]; requests and
+        expected_exact (scalars); request, the node ids of the request roots."""
+        from . import traces
+        need = {"chosen_score": "want_likelihood=True", "chosen_code": "want_likelihood=True",
+                "topk_score": "want_scores=True", "topk_idx": "want_scores=True", "topk_cnt": "want_scores=True",
+                "assign": "a solve() result"}
+        missing = [k for k in need if k not in out or out[k] is None]
+        if missing:
+            how = sorted({need[k] for k in missing})
+            raise ValueError(f"request_confidence: `out` lacks {', '.join(missing)}; call solve() with "
+                             f"{' and '.join(how)}")
+        eng = self.engine
+        res = traces.request_confidence(eng, hb, out["assign"], in_caller, out["chosen_score"], out["chosen_code"],
+                                        {k: out[k] for k in ("topk_score", "topk_idx", "topk_cnt")})
+        host = {k: v.cpu().numpy() for k, v in res.items()}
+        n_in = int(hb.prob_in_off[-1])
+        host["requests"] = int(host["requests"][0])
+        host["expected_exact"] = float(host["expected_exact"][0])
+        host["request"] = np.flatnonzero(host["root"][:n_in] == np.arange(n_in)).astype(np.int32)
+        return host

@@ -102,7 +102,8 @@ struct tw_engine {
   DevBuf<int32_t> trace_claim;
   DevBuf<int32_t> trace_flags;
   int trace_rounds_launched = 0, trace_rounds_run = 0, trace_still = 0;
-  // critical paths (tw_critical_paths): the join's parent and size words, the walk's scratch (CpScratch),
+  // critical paths (tw_critical_paths): the join's parent and size words (tw_request_confidence's too), the
+  // walk's scratch (CpScratch),
   // the level launches of the last call (tw_debug_critical_levels) and a forced level count, 0 = from the
   // rounds (tw_debug_critical_force_levels)
   DevBuf<int32_t> cp_parent;
@@ -114,6 +115,11 @@ struct tw_engine {
   DevBuf<unsigned long long> cp_cmax;
   DevBuf<int> cp_act;
   int cp_levels = 0, cp_force_levels = 0;
+  // request confidence (tw_request_confidence): CfScratch
+  DevBuf<unsigned long long> cf_wbits;
+  DevBuf<double> cf_seg_conf;
+  DevBuf<int32_t> cf_seg_req;
+  DevBuf<int32_t> cf_flag;
   // skip / cache mode scratch (tw_skip_solve)
   DevBuf<uint32_t> skip_sets;
   DevBuf<int64_t> skip_set_off;
@@ -803,6 +809,39 @@ int tw_critical_paths(tw_engine* eng, const tw_batch* dev, const tw_batch* h, co
   CpScratch sc{eng->cp_level.p, eng->cp_wlo.p, eng->cp_whi.p, eng->cp_slow.p, eng->cp_cmax.p, eng->cp_act.p};
   CU(launch_critical_paths(*dev, f64, assign, eng->trace_claim.p, eng->cp_parent.p, slow_us, *out, sc, levels,
                            eng->n_sm, s, eng->launches));
+  return TW_OK;
+}
+
+int tw_request_confidence(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const int32_t* assign,
+                          const int32_t* in_caller, const double* score, const uint8_t* code,
+                          const tw_score_out* top, const tw_confidence_out* out, void* stream_) {
+  if (!eng || !dev || !assign || !in_caller || !score || !code || !top || !top->topk_score || !top->topk_idx ||
+      !top->topk_cnt || !out || !out->root || !out->p || !out->ell || !out->decisions || !out->zero ||
+      !out->log_conf || !out->conf || !out->weakest || !out->weakest_p || !out->est_accuracy || !out->requests ||
+      !out->expected_exact)
+    return fail(TW_ERR_INVALID, "tw_request_confidence: NULL argument");
+  int rc = trace_check(h, "tw_request_confidence");
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream_;
+  CU(cudaSetDevice(eng->device));
+  const int64_t n_in = h->n_in_total, n_nodes = n_in + h->n_out_total;
+  CU(eng->cp_parent.reserve((size_t)n_nodes));
+  CU(eng->cp_size.reserve((size_t)n_nodes));
+  CU(eng->cf_wbits.reserve((size_t)n_in));
+  CU(eng->cf_seg_conf.reserve((size_t)h->n_problems));
+  CU(eng->cf_seg_req.reserve((size_t)h->n_problems));
+  CU(eng->cf_flag.reserve(1));
+  rc = trace_join(eng, dev, h, assign, in_caller, eng->cp_parent.p, out->root, eng->cp_size.p,
+                  "tw_request_confidence", s);
+  if (rc) return rc;
+  CfScratch sc{eng->cf_wbits.p, eng->cf_seg_conf.p, eng->cf_seg_req.p, eng->cf_flag.p};
+  CU(launch_request_confidence(*dev, assign, score, code, *top, *out, sc, eng->n_sm, s, eng->launches));
+  int32_t big = 0;
+  CU(cudaMemcpyAsync(&big, eng->cf_flag.p, sizeof big, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  if (big != 0x7f7f7f7f)
+    return fail(TW_ERR_RANGE_LIMIT, "tw_request_confidence: the request rooted at in-span node %s has 2^21 or more "
+                "decisions (its fixed-point sum could overflow)", std::to_string(big).c_str());
   return TW_OK;
 }
 

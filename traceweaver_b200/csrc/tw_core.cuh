@@ -1504,4 +1504,114 @@ TW_HD void cp_tail_walk(G& g, int32_t x) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Confidence of the reconstructed requests (tw_request_confidence, tw_confidence.cu).  exp and log are
+// written here from multiplications, additions and one division, each rounded once (dmul, dadd, dsub,
+// ddiv: never contracted), in a fixed order, and bit operations.  So the kernels, the CPU build and the
+// NumPy restatement (traces.conf_exp / conf_log) give the same bits; libdevice and the C library would not.
+// ---------------------------------------------------------------------------------------------
+TW_HD double conf_from_bits(uint64_t u) {
+  double d;
+  memcpy(&d, &u, sizeof d);
+  return d;
+}
+TW_HD uint64_t conf_bits(double d) {
+  uint64_t u;
+  memcpy(&u, &d, sizeof u);
+  return u;
+}
+
+#define TW_CONF_LN2_HI 0.6931471803691238      // ln 2, high 32 bits: k * hi is exact for |k| < 2^21
+#define TW_CONF_LN2_LO 1.9082149292705877e-10  // ln 2 - hi
+#define TW_CONF_RINT 6755399441055744.0        // 1.5 * 2^52: x + this - this = rint(x) for |x| < 2^51
+#define TW_CONF_FIX 4294967296.0               // 2^32: the fixed point of the request sums, in nats
+#define TW_CONF_MAX_DECISIONS (1 << 21)        // decisions per request the int64 sums hold
+
+// exp(d) for d <= 0 (0 below -746 and for NaN).  d = n ln2 + r with |r| <= ln2 / 2 (Cody-Waite), exp(r)
+// by Taylor's series to r^13 / 13!, then two exact scalings by powers of two (the second rounds once
+// where the result is subnormal).  Within 2 ulp of exp; exp(0) = 1 exactly.
+TW_HD double conf_exp(double d) {
+  if (!(d >= -746.0)) return 0.0;
+  const double nf = dsub(dadd(dmul(d, 1.4426950408889634), TW_CONF_RINT), TW_CONF_RINT);
+  const int n = (int)nf;
+  const double r = dsub(dsub(d, dmul(nf, TW_CONF_LN2_HI)), dmul(nf, TW_CONF_LN2_LO));
+  const double c[12] = {1.6059043836821613e-10, 2.08767569878681e-09, 2.505210838544172e-08,
+                        2.755731922398589e-07, 2.7557319223985893e-06, 2.48015873015873e-05,
+                        0.0001984126984126984, 0.001388888888888889, 0.008333333333333333,
+                        0.041666666666666664, 0.16666666666666666, 0.5};
+  double q = c[0];
+  for (int k = 1; k < 12; ++k) q = dadd(dmul(q, r), c[k]);
+  q = dadd(dmul(q, r), 1.0);
+  q = dadd(dmul(q, r), 1.0);
+  const int n1 = n >> 1, n2 = n - n1;              // n >= -1076: both factors are normal
+  return dmul(dmul(q, conf_from_bits((uint64_t)(n1 + 1023) << 52)), conf_from_bits((uint64_t)(n2 + 1023) << 52));
+}
+
+// log(x) for a positive normal x.  x = 2^k f with f in [sqrt(1/2), sqrt(2)); log f = 2 atanh(s),
+// s = (f - 1) / (f + 1), by its series to s^21 / 21.  Within 2 ulp of log; log(1) = 0 and log(x) >= 0 for
+// x >= 1.
+TW_HD double conf_log(double x) {
+  const uint64_t u = conf_bits(x);
+  int k = (int)(u >> 52) - 1023;
+  double f = conf_from_bits((u & 0x000fffffffffffffULL) | 0x3ff0000000000000ULL);
+  if (f > 1.4142135623730951) {
+    f = dmul(f, 0.5);
+    ++k;
+  }
+  const double s = ddiv(dsub(f, 1.0), dadd(f, 1.0));
+  const double z = dmul(s, s);
+  const double c[10] = {0.047619047619047616, 0.05263157894736842, 0.058823529411764705, 0.06666666666666667,
+                        0.07692307692307693, 0.09090909090909091, 0.1111111111111111, 0.14285714285714285,
+                        0.2, 0.3333333333333333};
+  double q = c[0];
+  for (int j = 1; j < 10; ++j) q = dadd(dmul(q, z), c[j]);
+  const double s2 = dadd(s, s);
+  const double lf = dadd(s2, dmul(dmul(s2, z), q));
+  return dadd(dmul((double)k, TW_CONF_LN2_HI), dadd(dmul((double)k, TW_CONF_LN2_LO), lf));
+}
+
+// One reconstruction decision: in-span x with feasibility code `code` and chosen tuple c[0..E) of score sc
+// (tw_score_assignments), and its final no-deletion top-K row: scores tks[r], tuples tki[r * E + e], cnt
+// listed ranks.  p is the chosen tuple's share of the likelihood among the alternatives the engine listed:
+// 0 unless code == TW_ASSESS_SCORED (and sc > -inf); else with A the listed ranks whose tuple differs from
+// c at some callee position and m = max(sc, max_A s_r),
+//   S = exp(sc - m) + sum over r in A, ascending, of exp(s_r - m),   p = exp(sc - m) / S.
+// ell = -log p, formed as log(S) + (m - sc) (no underflow on the way); +inf where p == 0.  q = ell in units
+// of 2^-32 nats, rounded to nearest even, -1 where p == 0.  A finite ell is below 748 (exp(sc - m) > 0 needs
+// m - sc <= 746, and S <= TW_K + 1), so q < 2^42.
+struct ConfChoice {
+  double p, ell;
+  int64_t q;
+};
+
+TW_HD ConfChoice conf_choice(int E, const int32_t* c, int code, double sc, const double* tks, const int32_t* tki,
+                             int cnt) {
+  ConfChoice o{0.0, INFINITY, -1};
+  if (code != TW_ASSESS_SCORED || !(sc > -INFINITY)) return o;
+  if (cnt > TW_K) cnt = TW_K;
+  bool alt[TW_K];
+  double m = sc;
+  for (int r = 0; r < cnt; ++r) {
+    bool same = true;
+    for (int e = 0; e < E; ++e) same = same && tki[r * E + e] == c[e];
+    alt[r] = !same;
+    if (alt[r] && tks[r] > m) m = tks[r];
+  }
+  const double a = conf_exp(dsub(sc, m));
+  double S = a;
+  for (int r = 0; r < cnt; ++r)
+    if (alt[r]) S = dadd(S, conf_exp(dsub(tks[r], m)));
+  const double p = ddiv(a, S);
+  if (!(p > 0.0)) return o;
+  o.p = p;
+  o.ell = dadd(conf_log(S), dsub(m, sc));
+  o.q = (int64_t)dsub(dadd(dmul(o.ell, TW_CONF_FIX), TW_CONF_RINT), TW_CONF_RINT);
+  return o;
+}
+
+// A request's confidence from its fixed-point sum lq (units of 2^-32 nats) and its count of p = 0 decisions.
+TW_HD double conf_request(int64_t lq, int zero) {
+  return zero > 0 ? 0.0 : conf_exp(dmul((double)lq, -1.0 / TW_CONF_FIX));
+}
+
 }  // namespace tw

@@ -280,4 +280,17 @@ cudaError_t launch_critical_paths(const tw_batch& b, const tw_times_f64* f64, co
                                   const tw_critical_out& out, const CpScratch& sc, int levels, int n_sm,
                                   cudaStream_t s, int64_t& launches);
 
+// tw_confidence.cu: the passes after the join.  Scratch: wbits [n_in] (smallest p bits of each request),
+// seg_conf / seg_req [P] (per-service partials of the batch total), flag [1] (the smallest root with
+// TW_CONF_MAX_DECISIONS or more decisions, 0x7f7f7f7f = none).
+struct CfScratch {
+  unsigned long long* wbits;
+  double* seg_conf;
+  int32_t* seg_req;
+  int32_t* flag;
+};
+cudaError_t launch_request_confidence(const tw_batch& b, const int32_t* assign, const double* score,
+                                      const uint8_t* code, const tw_score_out& top, const tw_confidence_out& out,
+                                      const CfScratch& sc, int n_sm, cudaStream_t s, int64_t& launches);
+
 }  // namespace tw

@@ -353,3 +353,223 @@ def critical_paths_host(hb, assign, in_caller, slow_us):
     return dict(root=root, on_path=on_path, self_us=self_us, culprit=culprit, server_us=server_us,
                 server_visits=server_visits, call_us=call_us,
                 requests=np.array([len(requests), int((latency >= slow_us).sum())], np.int32), latency=latency)
+
+
+# ---------------------------------------------------------------------------------------------
+# Request confidence (tw_request_confidence, csrc/tw_confidence.cu): how sure the reconstruction of each
+# request is, without a ground truth.  This is the project's own definition.  Every in-span x is one
+# reconstruction decision.  Its choice probability p_x is the chosen tuple's share of the likelihood among
+# the alternatives the engine listed:
+#   p_x = 0 unless code[x] == TW_ASSESS_SCORED (NA, out of range, infeasible; also when score[x] is -inf);
+#   else, with A the listed ranks r < topk_cnt[x] of the final no-deletion top-K whose tuple differs from
+#   the chosen one at some callee position, s_c = score[x] and m = max(s_c, max_A s_r):
+#     S = exp(s_c - m) + sum over r in A, ascending, of exp(s_r - m),   p_x = exp(s_c - m) / S.
+#   A single candidate gives 1; a chosen tuple the list does not hold counts with its own score.
+#   ell_x = -log p_x, formed as log(S) + (m - s_c); +inf where p_x == 0 (also when exp underflows).
+# It ignores the windows' conflicts and the tuples beyond rank K, so it is pessimistic: a ranking signal,
+# not a calibrated probability, and not an accuracy.  Per request r (an in-span root of the join; in-spans
+# on or under a cycle or in a detached fragment belong to none): decisions[r], zero[r] (decisions with
+# p = 0), log_conf[r] = the sum of the others' ell, each rounded to a multiple of 2^-32 nats and added as
+# int64; conf[r] = exp(-log_conf[r] * 2^-32), 0 when zero[r] > 0; weakest[r] the decision with the smallest
+# p (smallest node id on a tie) and weakest_p[r] its p.  Per service est_accuracy = the mean p of its
+# in-spans; per batch the request count and expected_exact = the sum of conf.  exp and log are the engine's
+# own (conf_exp / conf_log below, the same operations as tw_core.cuh), so every float here is bit-identical
+# to the device's; the sums follow the kernels' fixed order (_cta_sum).
+# ---------------------------------------------------------------------------------------------
+_CONF_KEYS = ("root", "p", "ell", "decisions", "zero", "log_conf", "conf", "weakest", "weakest_p", "est_accuracy",
+              "requests", "expected_exact")
+_LN2_HI, _LN2_LO, _RINT = 0.6931471803691238, 1.9082149292705877e-10, 6755399441055744.0
+_EXP_C = (1.6059043836821613e-10, 2.08767569878681e-09, 2.505210838544172e-08, 2.755731922398589e-07,
+          2.7557319223985893e-06, 2.48015873015873e-05, 0.0001984126984126984, 0.001388888888888889,
+          0.008333333333333333, 0.041666666666666664, 0.16666666666666666, 0.5, 1.0, 1.0)
+_LOG_C = (0.047619047619047616, 0.05263157894736842, 0.058823529411764705, 0.06666666666666667,
+          0.07692307692307693, 0.09090909090909091, 0.1111111111111111, 0.14285714285714285, 0.2,
+          0.3333333333333333)
+
+
+def conf_exp(d):
+    """exp(d) for d <= 0 as tw_core.cuh's conf_exp computes it (0 below -746 and for NaN), elementwise."""
+    d = np.asarray(d, np.float64)
+    ok = d >= -746.0
+    x = np.where(ok, d, 0.0)
+    nf = (x * 1.4426950408889634 + _RINT) - _RINT
+    r = (x - nf * _LN2_HI) - nf * _LN2_LO
+    q = np.full_like(x, _EXP_C[0])
+    for c in _EXP_C[1:]:
+        q = q * r + c
+    n = nf.astype(np.int64)
+    n1 = n >> 1
+    pow2 = lambda k: ((k + 1023) << 52).astype(np.int64).view(np.float64)
+    return np.where(ok, (q * pow2(n1)) * pow2(n - n1), 0.0)
+
+
+def conf_log(x):
+    """log(x) for positive normal x as tw_core.cuh's conf_log computes it, elementwise."""
+    u = np.asarray(x, np.float64).view(np.int64)
+    k = (u >> 52) - 1023
+    f = ((u & 0x000fffffffffffff) | 0x3ff0000000000000).view(np.float64)
+    big = f > 1.4142135623730951
+    f = np.where(big, f * 0.5, f)
+    k = k + big
+    s = (f - 1.0) / (f + 1.0)
+    z = s * s
+    q = np.full_like(s, _LOG_C[0])
+    for c in _LOG_C[1:]:
+        q = q * z + c
+    s2 = s + s
+    kf = k.astype(np.float64)
+    return kf * _LN2_HI + (kf * _LN2_LO + (s2 + (s2 * z) * q))
+
+
+def _cta_sum(v):
+    """The kernels' fixed-order sum of v (one CTA of 256 threads: thread t adds v[t], v[t + 256], ... in order,
+    a butterfly per warp of 32, then the warps in order)."""
+    v = np.asarray(v, np.float64)
+    lanes = np.zeros(256)
+    for lo in range(0, len(v), 256):
+        row = v[lo:lo + 256]
+        lanes[:len(row)] = lanes[:len(row)] + row
+    w = lanes.reshape(8, 32)
+    for d in (16, 8, 4, 2, 1):
+        w = w + w[:, np.arange(32) ^ d]
+    s = w[0, 0]
+    for k in range(1, 8):
+        s = s + w[k, 0]
+    return float(s)
+
+
+def _topk_arrays(topk, n_in, n_tuple):
+    sc = np.asarray(topk["topk_score"], np.float64).reshape(-1)
+    idx = np.asarray(topk["topk_idx"], np.int32).reshape(-1)
+    cnt = np.asarray(topk["topk_cnt"], np.uint8).reshape(-1)
+    if sc.size != _abi.TW_K * n_in or idx.size != _abi.TW_K * n_tuple or cnt.size != n_in:
+        raise ValueError(f"request_confidence: topk_score must have {_abi.TW_K * n_in} entries, topk_idx "
+                         f"{_abi.TW_K * n_tuple} and topk_cnt {n_in}")
+    return sc, idx, cnt
+
+
+def request_confidence(engine, hb, assign, in_caller, score, code, topk):
+    """tw_request_confidence on the batch `hb` (host offsets; it need not be bound, a bound batch is not
+    touched).  assign, in_caller as for assemble; score float64 / code uint8 [n_in] of the chosen tuples
+    (tw_score_assignments: solve(want_likelihood=True)'s chosen_score / chosen_code, or BatchSolver.score);
+    topk: topk_score [n_in, K], topk_idx, topk_cnt of the final no-deletion top-K (solve(want_scores=True)).
+    Device tensors or host arrays.  Returns device tensors: root int32 [N]; p, ell float64, decisions, zero
+    int32, log_conf int64 (units of 2^-32 nats), conf float64, weakest int32, weakest_p float64 [n_in];
+    est_accuracy float64 [P]; requests int32 [1]; expected_exact float64 [1].  Definition above."""
+    dev = engine.device
+    d = _to_device({k: hb.arrays[k] for k in _OFFSETS}, dev)
+    n_tuple, n_in = int(hb.prob_tuple_off[-1]), int(hb.prob_in_off[-1])
+    want = dict(assign=(n_tuple, np.int32, torch.int32), in_caller=(n_in, np.int32, torch.int32),
+                score=(n_in, np.float64, torch.float64), code=(n_in, np.uint8, torch.uint8),
+                topk_score=(_abi.TW_K * n_in, np.float64, torch.float64),
+                topk_idx=(_abi.TW_K * n_tuple, np.int32, torch.int32), topk_cnt=(n_in, np.uint8, torch.uint8))
+    given = dict(assign=assign, in_caller=in_caller, score=score, code=code, topk_score=topk["topk_score"],
+                 topk_idx=topk["topk_idx"], topk_cnt=topk["topk_cnt"])
+    links = {}
+    for name, a in given.items():
+        size, npt, tt = want[name]
+        if isinstance(a, torch.Tensor):
+            t = a.to(device=dev, dtype=tt).contiguous().reshape(-1)
+        else:
+            t = _to_device({name: np.ascontiguousarray(np.asarray(a, npt).reshape(-1))}, dev)[name]
+        if t.numel() != size:
+            raise ValueError(f"request_confidence: {name} must have {size} entries for this batch, not {t.numel()}")
+        links[name] = t
+    view = _OffsetView(hb)
+    dev_s = batch_struct(view, lambda k: d[k].data_ptr())
+    host_s = batch_struct(view, lambda k: hb.arrays[k].ctypes.data)
+    n, P = node_count(hb), hb.n_problems
+    out = dict(root=torch.empty(n, dtype=torch.int32, device=dev))
+    for k, dt in (("p", torch.float64), ("ell", torch.float64), ("decisions", torch.int32), ("zero", torch.int32),
+                  ("log_conf", torch.int64), ("conf", torch.float64), ("weakest", torch.int32),
+                  ("weakest_p", torch.float64)):
+        out[k] = torch.empty(n_in, dtype=dt, device=dev)
+    out.update(est_accuracy=torch.empty(P, dtype=torch.float64, device=dev),
+               requests=torch.empty(1, dtype=torch.int32, device=dev),
+               expected_exact=torch.empty(1, dtype=torch.float64, device=dev))
+    top = _abi.fill(_abi.TwScoreOut, {k: links[k] for k in ("topk_score", "topk_idx", "topk_cnt")})
+    o = _abi.fill(_abi.TwConfidenceOut, out)
+    _lib.check(engine.lib.tw_request_confidence(engine.h, C.byref(dev_s), C.byref(host_s), _p(links["assign"]),
+                                                _p(links["in_caller"]), _p(links["score"]), _p(links["code"]),
+                                                C.byref(top), C.byref(o), engine.stream), "tw_request_confidence")
+    return out
+
+
+def choice_host(hb, assign, score, code, topk):
+    """p, ell (float64 [n_in]) and the fixed-point ell (int64, -1 where p == 0) of every in-span, as defined
+    above (vectorised over the in-spans of each service)."""
+    n_in, n_tuple = int(hb.prob_in_off[-1]), int(hb.prob_tuple_off[-1])
+    K = _abi.TW_K
+    tks, tki, cnt = _topk_arrays(topk, n_in, n_tuple)
+    tks = tks.reshape(n_in, K)
+    assign = np.asarray(assign, np.int32).reshape(-1)
+    score = np.asarray(score, np.float64).reshape(-1)
+    code = np.asarray(code, np.uint8).reshape(-1)
+    if assign.size != n_tuple or score.size != n_in or code.size != n_in:
+        raise ValueError(f"request_confidence: assign must have {n_tuple} entries, score and code {n_in}")
+    p_out = np.zeros(n_in)
+    ell = np.full(n_in, np.inf)
+    q = np.full(n_in, -1, np.int64)
+    for pb in range(hb.n_problems):
+        i0, i1 = int(hb.prob_in_off[pb]), int(hb.prob_in_off[pb + 1])
+        n, E = i1 - i0, int(hb.prob_ep_off[pb + 1] - hb.prob_ep_off[pb])
+        t0 = int(hb.prob_tuple_off[pb])
+        chosen = assign[t0:t0 + n * E].reshape(E, n).T                       # [n, E]
+        idx = tki[K * t0:K * (t0 + n * E)].reshape(n, K, E)
+        c = np.minimum(cnt[i0:i1], K)
+        s_c = score[i0:i1]
+        live = (code[i0:i1] == _abi.TW_ASSESS_SCORED) & (s_c > -np.inf)
+        alt = (idx != chosen[:, None, :]).any(axis=2) & (np.arange(K)[None, :] < c[:, None])
+        s = tks[i0:i1]
+        m = s_c.copy()
+        for r in range(K):
+            m = np.where(alt[:, r] & (s[:, r] > m), s[:, r], m)
+        a = conf_exp(np.where(live, s_c - m, 0.0))
+        S = a.copy()
+        for r in range(K):
+            S = np.where(alt[:, r], S + conf_exp(np.where(alt[:, r], s[:, r] - m, 0.0)), S)
+        pp = np.where(live, a / np.where(live, S, 1.0), 0.0)
+        pos = pp > 0.0
+        lg = conf_log(np.where(pos, S, 1.0)) + np.where(pos, m - s_c, 0.0)
+        p_out[i0:i1] = np.where(pos, pp, 0.0)
+        ell[i0:i1] = np.where(pos, lg, np.inf)
+        q[i0:i1] = np.where(pos, ((np.where(pos, lg, 0.0) * 4294967296.0 + _RINT) - _RINT).astype(np.int64), -1)
+    return p_out, ell, q
+
+
+def request_confidence_host(hb, assign, in_caller, score, code, topk):
+    """The arrays of request_confidence (numpy) from the definition above, with the join of assemble_host;
+    ValueError where tw_request_confidence returns TW_ERR_INVALID or TW_ERR_RANGE_LIMIT.  Also q, the
+    fixed-point ell of every in-span (-1 where p == 0)."""
+    _, root, _ = assemble_host(hb, assign, in_caller)
+    n_in, P = int(hb.prob_in_off[-1]), hb.n_problems
+    p, ell, q = choice_host(hb, assign, score, code, topk)
+    r = root[:n_in].astype(np.int64)
+    mine = (r >= 0) & (r < n_in)
+    decisions = np.bincount(r[mine], minlength=n_in).astype(np.int32)
+    zero = np.bincount(r[mine & (q < 0)], minlength=n_in).astype(np.int32)
+    log_conf = np.zeros(n_in, np.int64)
+    np.add.at(log_conf, r[mine & (q >= 0)], q[mine & (q >= 0)])
+    big = np.flatnonzero(decisions >= 1 << 21)
+    if big.size:
+        raise ValueError(f"the request rooted at in-span node {big[0]} has 2^21 or more decisions")
+    is_root = r == np.arange(n_in)
+    conf = np.full(n_in, np.nan)
+    conf[is_root] = np.where(zero[is_root] > 0, 0.0, conf_exp(log_conf[is_root].astype(np.float64) * -2.0 ** -32))
+    weakest = np.full(n_in, -1, np.int32)
+    weakest_p = np.full(n_in, np.nan)
+    x = np.flatnonzero(mine)
+    order = np.lexsort((x, p[x], r[x]))                   # by request, then p, then node id
+    xs = x[order]
+    first = np.ones(len(xs), bool)
+    first[1:] = r[xs][1:] != r[xs][:-1]
+    weakest[r[xs[first]]] = xs[first]
+    weakest_p[r[xs[first]]] = p[xs[first]]
+    est = np.array([_cta_sum(p[int(hb.prob_in_off[k]):int(hb.prob_in_off[k + 1])]) /
+                    float(hb.prob_in_off[k + 1] - hb.prob_in_off[k]) for k in range(P)])
+    seg_conf = [_cta_sum(np.where(is_root, conf, 0.0)[int(hb.prob_in_off[k]):int(hb.prob_in_off[k + 1])])
+                for k in range(P)]
+    return dict(root=root, p=p, ell=ell, decisions=decisions, zero=zero, log_conf=log_conf, conf=conf,
+                weakest=weakest, weakest_p=weakest_p, est_accuracy=est,
+                requests=np.array([int(is_root.sum())], np.int32), expected_exact=np.array([_cta_sum(seg_conf)]),
+                q=q)
