@@ -32,6 +32,7 @@ constexpr double kKmTol = 1e-4;
 constexpr double kDblEps = 2.220446049250313e-16;
 constexpr int KC = TW_GMM_MAX_COMP;
 constexpr unsigned kFull = 0xffffffffu;
+constexpr int kLloydLabelN = 1024;   // longest sample list whose Lloyd labels stay in shared memory
 
 // optional phase timers (build with -DTW_PROFILE_PHASES; scripts/phase_profile.py reads them):
 // cycles in seeding / Lloyd / initial M-step / EM / scoring, then Lloyd and EM iteration counts, fits
@@ -72,9 +73,10 @@ __device__ __forceinline__ double wsum(double v) {
 __device__ __forceinline__ int trials_for_k(int k) { return k < 3 ? 2 : 3; }
 __device__ __forceinline__ int draws_for_k(int k) { return 1 + (k - 1) * trials_for_k(k); }
 
-// _euclidean_distances(squared=True): -2 c x + c^2 + x^2, clipped at 0
+// _euclidean_distances(squared=True): -2 c x + c^2 + x^2, clipped at 0.  The product by -2 is exact,
+// so the fused form rounds the same sum as dadd(dmul(-2.0, dmul(c, x)), c2).
 __device__ __forceinline__ double sq_dist(double c, double c2, double x, double x2) {
-  double d = dadd(dadd(dmul(-2.0, dmul(c, x)), c2), x2);
+  double d = dadd(__fma_rn(-2.0, dmul(c, x), c2), x2);
   return d > 0.0 ? d : 0.0;
 }
 
@@ -86,16 +88,22 @@ struct Fit {
 
 // arg-min over centres of c^2 - 2 x c (the x^2 term is common), first minimum wins — evaluated as a
 // tree (depth 3 for K = 5) instead of a chain; strict "<" with the lower index on the left keeps
-// NumPy's tie rule.
+// NumPy's tie rule.  cen2[j] = dmul(cen[j], cen[j]), computed once per set of centres; the product
+// by -2 is exact, so the fused form rounds the same sum as dadd(cen2[j], dmul(-2.0, dmul(x, cen[j]))).
 struct Near { double d; int j; };
 __device__ __forceinline__ Near near_min(Near a, Near b) { return b.d < a.d ? b : a; }
 template <int K>
-__device__ __forceinline__ int nearest(const double* cen, double x) {
+__device__ __forceinline__ void centre_squares(const double* cen, double* cen2) {
+#pragma unroll
+  for (int j = 0; j < KC; ++j) cen2[j] = j < K ? dmul(cen[j], cen[j]) : 0.0;
+}
+template <int K>
+__device__ __forceinline__ int nearest(const double* cen, const double* cen2, double x) {
   Near v[KC];
 #pragma unroll
   for (int j = 0; j < KC; ++j) {
     v[j].j = j;
-    v[j].d = j < K ? dadd(dmul(cen[j], cen[j]), dmul(-2.0, dmul(x, cen[j]))) : 0.0;
+    v[j].d = j < K ? __fma_rn(-2.0, dmul(x, cen[j]), cen2[j]) : 0.0;
   }
   if (K == 1) return 0;
   if (K == 2) return near_min(v[0], v[1]).j;
@@ -122,9 +130,8 @@ __device__ __forceinline__ void sweep2(const double* __restrict__ x, int n, F&& 
   }
 }
 
-// KMeans(n_clusters=k, n_init=1).fit(X): returns the centres (on centred data) that define the
-// final labels_.  draws[] = this fit's random_sample() values.
 // k-means++ seeding of KMeans(n_clusters=K, n_init=1).fit(X) on centred data (x - mean).
+// draws[] = this fit's random_sample() values.
 template <int K>
 __device__ __forceinline__ void seed_centres(const double* __restrict__ x, int n, double mean,
                                              const double* __restrict__ draws, double* cen) {
@@ -138,28 +145,28 @@ __device__ __forceinline__ void seed_centres(const double* __restrict__ x, int n
   // within rounding of an integer, in which case the sequential sum is replayed exactly.
   {
     double u = draws[0];
-    double un = u * (double)n;
+    double un = dmul(u, (double)n);
     int id = (int)un;
-    if (fabs(un - rint(un)) < 1e-6) {
+    if (fabs(dsub(un, rint(un))) < 1e-6) {
       double p = 1.0 / (double)n, last = 0.0, c = 0.0;
-      for (int i = 0; i < n; ++i) last += p;
+      for (int i = 0; i < n; ++i) last = dadd(last, p);
       id = n - 1;
-      for (int i = 0; i < n; ++i) { c += p; if (c / last > u) { id = i; break; } }
+      for (int i = 0; i < n; ++i) { c = dadd(c, p); if (c / last > u) { id = i; break; } }
     }
     if (id > n - 1) id = n - 1;
-    cen[0] = x[id] - mean;
+    cen[0] = dsub(x[id], mean);
   }
   const int trials = trials_for_k(k);
   double pot = 0.0;
   {
-    double part = 0.0, c2 = cen[0] * cen[0];
-    for (int i = lane; i < n; i += 32) { double xi = x[i] - mean; part += sq_dist(cen[0], c2, xi, xi * xi); }
+    double part = 0.0, c2 = dmul(cen[0], cen[0]);
+    for (int i = lane; i < n; i += 32) { double xi = dsub(x[i], mean); part = dadd(part, sq_dist(cen[0], c2, xi, dmul(xi, xi))); }
     pot = wsum(part);
   }
   for (int ci = 1; ci < k; ++ci) {
     double rv[3];
     int cand[3];
-    for (int t = 0; t < 3; ++t) { rv[t] = t < trials ? draws[1 + (ci - 1) * trials + t] * pot : 0.0; cand[t] = n - 1; }
+    for (int t = 0; t < 3; ++t) { rv[t] = t < trials ? dmul(draws[1 + (ci - 1) * trials + t], pot) : 0.0; cand[t] = n - 1; }
     bool found[3] = {false, false, false};
     // np.searchsorted(np.cumsum(closest), rv): first i with cumsum_i >= rv, rounds of 32 samples
     double carry = 0.0;
@@ -167,17 +174,17 @@ __device__ __forceinline__ void seed_centres(const double* __restrict__ x, int n
       int i = base + lane;
       double cl = 0.0;
       if (i < n) {
-        double xi = x[i] - mean, x2 = xi * xi;
-        cl = sq_dist(cen[0], cen[0] * cen[0], xi, x2);
-        for (int j = 1; j < ci; ++j) { double d = sq_dist(cen[j], cen[j] * cen[j], xi, x2); cl = d < cl ? d : cl; }
+        double xi = dsub(x[i], mean), x2 = dmul(xi, xi);
+        cl = sq_dist(cen[0], dmul(cen[0], cen[0]), xi, x2);
+        for (int j = 1; j < ci; ++j) { double d = sq_dist(cen[j], dmul(cen[j], cen[j]), xi, x2); cl = d < cl ? d : cl; }
       }
       double incl = cl;
 #pragma unroll
       for (int d = 1; d < 32; d <<= 1) {
         double o = __shfl_up_sync(kFull, incl, d);
-        if (lane >= d) incl += o;
+        if (lane >= d) incl = dadd(incl, o);
       }
-      incl += carry;
+      incl = dadd(incl, carry);
       for (int t = 0; t < trials; ++t) {
         if (found[t]) continue;
         unsigned m = __ballot_sync(kFull, i < n && incl >= rv[t]);
@@ -187,14 +194,14 @@ __device__ __forceinline__ void seed_centres(const double* __restrict__ x, int n
       if (found[0] && (trials < 2 || found[1]) && (trials < 3 || found[2])) break;
     }
     double cc[3], part[3] = {0.0, 0.0, 0.0};
-    for (int t = 0; t < 3; ++t) cc[t] = x[cand[t]] - mean;
+    for (int t = 0; t < 3; ++t) cc[t] = dsub(x[cand[t]], mean);
     for (int i = lane; i < n; i += 32) {
-      double xi = x[i] - mean, x2 = xi * xi;
-      double cl = sq_dist(cen[0], cen[0] * cen[0], xi, x2);
-      for (int j = 1; j < ci; ++j) { double d = sq_dist(cen[j], cen[j] * cen[j], xi, x2); cl = d < cl ? d : cl; }
+      double xi = dsub(x[i], mean), x2 = dmul(xi, xi);
+      double cl = sq_dist(cen[0], dmul(cen[0], cen[0]), xi, x2);
+      for (int j = 1; j < ci; ++j) { double d = sq_dist(cen[j], dmul(cen[j], cen[j]), xi, x2); cl = d < cl ? d : cl; }
       for (int t = 0; t < trials; ++t) {
-        double d = sq_dist(cc[t], cc[t] * cc[t], xi, x2);
-        part[t] += d < cl ? d : cl;
+        double d = sq_dist(cc[t], dmul(cc[t], cc[t]), xi, x2);
+        part[t] = dadd(part[t], d < cl ? d : cl);
       }
     }
     int best = 0;
@@ -210,9 +217,10 @@ __device__ __forceinline__ void seed_centres(const double* __restrict__ x, int n
 }
 
 // Lloyd iterations from the seeded centres: cen[] in, the centres that define the final labels_ out.
+// labs = this warp's kLloydLabelN bytes of shared memory.
 template <int K>
 __device__ __forceinline__ void lloyd_centres(const double* __restrict__ x, int n, double mean, double tol,
-                                              const double* cen_in, double* cen_out) {
+                                              const double* cen_in, double* cen_out, unsigned char* labs) {
   const int lane = threadIdx.x & 31;
   const int k = K;
   TW_GPHASE_BEGIN;
@@ -220,76 +228,85 @@ __device__ __forceinline__ void lloyd_centres(const double* __restrict__ x, int 
 #pragma unroll
   for (int j = 0; j < KC; ++j) cen[j] = cen_in[j];
   // ---- Lloyd (_kmeans_single_lloyd).  The labels of the previous assignment (needed for the
-  // "no label changed" stop) live in two packed registers per lane when n <= 1024 (4 bits per
-  // sample, 32 samples per lane); longer sample lists recompute them from the previous centres.
-  double prev[KC];
+  // "no label changed" stop) live in one shared-memory byte per sample when n <= kLloydLabelN;
+  // sample i is only ever read and written by lane i % 32.  Longer sample lists recompute them from
+  // the previous centres.  With at most 32 samples per lane, a lane's K counts fit in 6-bit fields
+  // of one word.
+  double prev[KC], cen2[KC];
 #pragma unroll
   for (int j = 0; j < KC; ++j) prev[j] = cen[j];
   bool have_prev = false, strict = false;
-  const bool packed = n <= 1024;
-  unsigned long long lab_lo = 0ull, lab_hi = 0ull;
+  const bool packed = n <= kLloydLabelN;
   for (int it = 0; it < kKmMaxIter; ++it) {
     double sx[KC];
     int cnt_i[KC];
 #pragma unroll
     for (int j = 0; j < KC; ++j) { sx[j] = 0.0; cnt_i[j] = 0; }
     bool changed = !have_prev;
+    centre_squares<K>(cen, cen2);
     if (packed) {
+      unsigned cnt_p = 0u;
       sweep2(x, n, [&](double x0, double x1, bool v1, int s) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const double xi = (h ? x1 : x0) - mean;
+          const double xi = dsub(h ? x1 : x0, mean);
           const bool valid = h ? v1 : true;
-          const int lab = nearest<K>(cen, xi);
-          const int sl = s + h;
-          const unsigned sh = (unsigned)(sl & 15) * 4u;
-          const bool hi = sl >= 16;
-          const unsigned long long w = hi ? lab_hi : lab_lo;
-          changed |= valid && (int)((w >> sh) & 15ull) != lab;      // first sweep: forced true below
-          const unsigned long long nw = valid ? (w & ~(15ull << sh)) | ((unsigned long long)lab << sh) : w;
-          lab_lo = hi ? lab_lo : nw;
-          lab_hi = hi ? nw : lab_hi;
-#pragma unroll
-          for (int j = 0; j < K; ++j) {
-            const bool m = valid && j == lab;
-            sx[j] += m ? xi : 0.0;
-            cnt_i[j] += m ? 1 : 0;
+          const int lab = nearest<K>(cen, cen2, xi);
+          if (valid) {
+            unsigned char& old = labs[lane + 32 * (s + h)];
+            changed |= have_prev && old != lab;                     // first sweep: forced true below
+            old = (unsigned char)lab;
+            cnt_p += 1u << (6 * lab);
           }
+#pragma unroll
+          for (int j = 0; j < K; ++j) sx[j] = dadd(sx[j], valid && j == lab ? xi : 0.0);
         }
       });
+#pragma unroll
+      for (int j = 0; j < K; ++j) cnt_i[j] = (int)((cnt_p >> (6 * j)) & 63u);
     } else {
+      double prev2[KC];
+      centre_squares<K>(prev, prev2);
       for (int i = lane; i < n; i += 32) {
-        const double xi = x[i] - mean;
-        const int lab = nearest<K>(cen, xi);
-        if (have_prev && nearest<K>(prev, xi) != lab) changed = true;
+        const double xi = dsub(x[i], mean);
+        const int lab = nearest<K>(cen, cen2, xi);
+        if (have_prev && nearest<K>(prev, prev2, xi) != lab) changed = true;
 #pragma unroll
         for (int j = 0; j < K; ++j) {
           const bool m = j == lab;
-          sx[j] += m ? xi : 0.0;
+          sx[j] = dadd(sx[j], m ? xi : 0.0);
           cnt_i[j] += m ? 1 : 0;
         }
       }
     }
     if (!have_prev) changed = true;
+    // the K count reductions, the K sum butterflies (each in wsum's order) and the vote are
+    // independent: issued together, their latencies overlap
     double cnt[KC];
 #pragma unroll
-    for (int j = 0; j < KC; ++j) cnt[j] = (double)__reduce_add_sync(kFull, cnt_i[j]);
+    for (int j = 0; j < KC; ++j) cnt[j] = j < K ? (double)__reduce_add_sync(kFull, cnt_i[j]) : 0.0;
     changed = __any_sync(kFull, changed);
 #pragma unroll
-    for (int j = 0; j < KC; ++j) sx[j] = wsum(sx[j]);
+    for (int d = 16; d > 0; d >>= 1) {
+#pragma unroll
+      for (int j = 0; j < K; ++j) sx[j] += __shfl_xor_sync(kFull, sx[j], d);
+    }
     // _relocate_empty_clusters_dense (rare): farthest point from its centre moves to the empty cluster
     for (int j = 0; j < k; ++j) {
-      if (cnt[j] != 0.0) continue;
+      bool empty = false;          // cnt[j] == 0, selected without indexing cnt[] by a run-time j
+#pragma unroll
+      for (int q = 0; q < K; ++q) empty = q == j ? cnt[q] == 0.0 : empty;
+      if (!empty) continue;
       double fd = -1.0;
       int fi = 0x7fffffff;
       for (int i = lane; i < n; i += 32) {
-        double xi = x[i] - mean;
-        const int nl = nearest<K>(cen, xi);
+        double xi = dsub(x[i], mean);
+        const int nl = nearest<K>(cen, cen2, xi);
         double cn = cen[0];
 #pragma unroll
         for (int q = 1; q < KC; ++q) cn = q == nl ? cen[q] : cn;
-        double d = xi - cn;
-        d *= d;
+        double d = dsub(xi, cn);
+        d = dmul(d, d);
         if (d > fd) { fd = d; fi = i; }
       }
 #pragma unroll
@@ -298,11 +315,11 @@ __device__ __forceinline__ void lloyd_centres(const double* __restrict__ x, int 
         int oi = __shfl_xor_sync(kFull, fi, d);
         if (od > fd || (od == fd && oi < fi)) { fd = od; fi = oi; }
       }
-      double xf = x[fi] - mean;
-      int ol = nearest<K>(cen, xf);
+      double xf = dsub(x[fi], mean);
+      int ol = nearest<K>(cen, cen2, xf);
 #pragma unroll
       for (int q = 0; q < KC; ++q) {
-        if (q == ol) { sx[q] -= xf; cnt[q] -= 1.0; }
+        if (q == ol) { sx[q] = dsub(sx[q], xf); cnt[q] -= 1.0; }
         if (q == j) { sx[q] = xf; cnt[q] = 1.0; }
       }
     }
@@ -311,9 +328,9 @@ __device__ __forceinline__ void lloyd_centres(const double* __restrict__ x, int 
     for (int j = 0; j < KC; ++j) {
       prev[j] = cen[j];
       if (j < k) {
-        double nc = cnt[j] > 0.0 ? sx[j] * (1.0 / cnt[j]) : sx[j];
-        double d = fabs(nc - cen[j]);
-        shift_tot += d * d;
+        double nc = cnt[j] > 0.0 ? dmul(sx[j], 1.0 / cnt[j]) : sx[j];
+        double d = fabs(dsub(nc, cen[j]));
+        shift_tot = __fma_rn(d, d, shift_tot);
         cen[j] = nc;
       }
     }
@@ -383,10 +400,6 @@ __device__ __forceinline__ double estep(const Fit& f, const double* __restrict__
   double amax = -INFINITY;
 #pragma unroll
   for (int c = 0; c < K; ++c) {
-#ifdef TW_GMM_FUSED
-    const double y = (x - f.mu[c]) * f.pc[c];
-    a[c] = fma(-0.5 * y, y, (f.logpc[c] - 0.5 * TW_LOG_2PI) + f.logw[c]);
-#else
     double lp;
     if (FULL) {
       double y = dsub(dmul(x, f.pc[c]), dmul(f.mu[c], f.pc[c]));
@@ -397,7 +410,6 @@ __device__ __forceinline__ double estep(const Fit& f, const double* __restrict__
                 dmul(dmul(x, x), prec));
     }
     a[c] = dadd(dadd(dmul(-0.5, dadd(TW_LOG_2PI, lp)), f.logpc[c]), f.logw[c]);
-#endif
     amax = a[c] > amax ? a[c] : amax;
   }
   double t = 0.0;
@@ -440,6 +452,8 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
   double my_nk, my_mup, my_s2;       // this lane's component (lanes 0..K-1)
   TW_GPHASE_BEGIN;
   {
+    double cen2[KC];
+    centre_squares<K>(cen, cen2);
     TW_GCOUNT(7, 1);
 #pragma unroll
     for (int c = 0; c < KC; ++c) { S0[c] = 0.0; S1[c] = 0.0; S2[c] = 0.0; }
@@ -447,7 +461,7 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const double xi = h ? x1 : x0;
-        const int lab = (h ? v1 : true) ? nearest<K>(cen, xi - mean) : -1;
+        const int lab = (h ? v1 : true) ? nearest<K>(cen, cen2, xi - mean) : -1;
         const double xs = xi - shift, xs2 = xs * xs;
 #pragma unroll
         for (int c = 0; c < K; ++c) {
@@ -475,7 +489,7 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const double xi = h ? x1 : x0;
-          const int lab = (h ? v1 : true) ? nearest<K>(cen, xi - mean) : -1;
+          const int lab = (h ? v1 : true) ? nearest<K>(cen, cen2, xi - mean) : -1;
           const double xs = xi - shift;
 #pragma unroll
           for (int c = 0; c < K; ++c) {
@@ -663,6 +677,9 @@ __global__ void k_gmm_draws(int n_problems, const int32_t* __restrict__ prob_ep_
 // Blocks of 128 threads per SM that the EM kernels are compiled for: 4 (16 warps) for K = 4, 5, whose
 // register footprint would otherwise allow only 3; the smaller K reach 16 warps unconstrained.
 constexpr int em_min_blocks(int K) { return K >= 4 ? 4 : 1; }
+// Blocks per SM that the Lloyd kernels are compiled for: 12, 8, 8, 7, 6 for K = 1..5 (at most 40, 64,
+// 64, 72, 80 registers, no spills).
+constexpr int lloyd_min_blocks(int K) { return K == 1 ? 12 : K == 2 ? 8 : K == 3 ? 8 : K == 4 ? 7 : 6; }
 
 // Which fit a warp works on.  Model selection (list == nullptr): warp w -> term w, active iff the
 // reference tries K components for it (K <= min(#unique, 5)), draws at the term's stream position.
@@ -718,7 +735,10 @@ k_gmm_seed(FitSel sel, const int64_t* __restrict__ term_sample_off, const double
            int* __restrict__ err_flag) {
   int t;
   const double* draws;
-  if (!select_fit<K>(sel, counts, &t, &draws, err_flag)) return;
+  if (!select_fit<K>(sel, counts, &t, &draws, err_flag)) return;   // flags a stream overrun for every K
+  // A 1-component fit labels every sample 0 whatever the centre (nearest<1>), so em_fit never reads
+  // the k-means result of K = 1: its seeding and Lloyd kernels have nothing more to do.
+  if (K == 1) return;
   double cen[KC];
   seed_centres<K>(delays + term_sample_off[t], counts[t], mean_var[2 * t], draws, cen);
   if ((threadIdx.x & 31) == 0) {
@@ -728,16 +748,19 @@ k_gmm_seed(FitSel sel, const int64_t* __restrict__ term_sample_off, const double
 }
 
 template <int K>
-__global__ void __launch_bounds__(128)
+__global__ void __launch_bounds__(128, lloyd_min_blocks(K))
 k_gmm_lloyd(FitSel sel, const int64_t* __restrict__ term_sample_off, const double* __restrict__ delays,
             const int32_t* __restrict__ counts, const double* __restrict__ mean_var, double* __restrict__ cen_io) {
+  if (K == 1) return;                    // see k_gmm_seed
   int t;
   const double* draws;
   if (!select_fit<K>(sel, counts, &t, &draws, nullptr)) return;
+  __shared__ unsigned char labs[128 / 32 * kLloydLabelN];
   double cen[KC], out[KC];
 #pragma unroll
   for (int j = 0; j < KC; ++j) cen[j] = j < K ? cen_io[(size_t)t * KC + j] : 0.0;
-  lloyd_centres<K>(delays + term_sample_off[t], counts[t], mean_var[2 * t], mean_var[2 * t + 1] * kKmTol, cen, out);
+  lloyd_centres<K>(delays + term_sample_off[t], counts[t], mean_var[2 * t], mean_var[2 * t + 1] * kKmTol, cen, out,
+                   labs + (threadIdx.x >> 5) * kLloydLabelN);
   if ((threadIdx.x & 31) == 0) {
 #pragma unroll
     for (int j = 0; j < K; ++j) cen_io[(size_t)t * KC + j] = out[j];
