@@ -13,7 +13,7 @@
 
 using namespace tw;
 
-// cf_cta_sum of tw_confidence.cu over v[0 .. n)
+// tree_cta_sum (tw_kernels.cuh) over v[0 .. n)
 static double cta_sum(const double* v, int64_t n) {
   double lane[256] = {0.0}, y[32];
   for (int t = 0; t < 256; ++t)

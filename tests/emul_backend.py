@@ -1,5 +1,6 @@
 """ctypes front end of tests/emul/libtw_emul.so: the engine's device functions (tw_core.cuh,
-tw_skip_core.cuh) compiled for the CPU and stepped sequentially.  Test infrastructure only."""
+tw_skip_core.cuh) compiled for the CPU and stepped sequentially (tw_emul.cpp; the request-tree analyses in
+tw_emul_critical.cpp and tw_emul_confidence.cpp).  Test infrastructure only."""
 import ctypes as C
 import os
 import subprocess
@@ -8,6 +9,7 @@ import numpy as np
 
 from oracle.tw_oracle import OracleBatch, _ptr, _check
 from traceweaver_b200 import _abi
+from traceweaver_b200.batch import HostBatch, batch_struct
 
 HERE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "emul")
 _LIB = None
@@ -156,3 +158,64 @@ def skip_score(in_start, in_end, out_start, out_end, preds, assign, wins, counts
     if top2 is not None:
         out["margin"] = res["margin"]
     return out
+
+
+def _host_struct(hb):
+    a = {k: np.ascontiguousarray(v) for k, v in hb.arrays.items()}
+    return a, batch_struct(HostBatch(problems=hb.problems, arrays=a), lambda k: a[k].ctypes.data)
+
+
+def critical_paths(hb, assign, in_caller, root, slow_us, levels=0):
+    """The critical-path walk with the kernels' per-node steps, stepped on the CPU; the join's roots come in.
+    levels: the level launches, the last of them walking what lies below it (cp_tail_walk); 0: until nothing
+    is left."""
+    a, st = _host_struct(hb)
+    times = _abi.fill(_abi.TwTimesF64, a) if hb.float_times else None
+    n_in, n = int(hb.prob_in_off[-1]), int(hb.prob_in_off[-1]) + int(hb.ep_out_off[-1])
+    P, n_ep = hb.n_problems, int(hb.prob_ep_off[-1])
+    out = dict(on_path=np.zeros(n, np.uint8), self_us=np.zeros(n), culprit=np.zeros(n_in, np.int32),
+               server_us=np.zeros((P, 2)), server_visits=np.zeros((P, 2), np.int32), call_us=np.zeros((n_ep, 2)),
+               requests=np.zeros(2, np.int32))
+    links = [np.ascontiguousarray(x, np.int32).reshape(-1) for x in (assign, in_caller, root)]
+    rc = lib().twe_critical_paths(C.byref(st), C.byref(times) if times is not None else None,
+                                  *[_ptr(x) for x in links], C.c_double(slow_us), C.c_int(levels),
+                                  *[_ptr(out[k]) for k in ("on_path", "self_us", "culprit", "server_us",
+                                                           "server_visits", "call_us", "requests")])
+    assert rc == 0
+    out["root"] = links[2]
+    return out
+
+
+def request_confidence(hb, assign, root, score, code, topk):
+    """The step, the per-request passes and the fixed-order sums of tw_confidence.cu stepped on the CPU; the
+    join's roots come in.  Returns the arrays and the return code."""
+    _, st = _host_struct(hb)
+    n_in, P = int(hb.prob_in_off[-1]), hb.n_problems
+    ins = [np.ascontiguousarray(np.asarray(x, t).reshape(-1)) for x, t in
+           ((assign, np.int32), (root, np.int32), (score, np.float64), (code, np.uint8),
+            (topk["topk_score"], np.float64), (topk["topk_idx"], np.int32), (topk["topk_cnt"], np.uint8))]
+    out = dict(p=np.zeros(n_in), ell=np.zeros(n_in), q=np.zeros(n_in, np.int64), decisions=np.zeros(n_in, np.int32),
+               zero=np.zeros(n_in, np.int32), log_conf=np.zeros(n_in, np.int64), conf=np.zeros(n_in),
+               weakest=np.zeros(n_in, np.int32), weakest_p=np.zeros(n_in), est_accuracy=np.zeros(P),
+               requests=np.zeros(1, np.int32), expected_exact=np.zeros(1))
+    order = ("p", "ell", "q", "decisions", "zero", "log_conf", "conf", "weakest", "weakest_p", "est_accuracy",
+             "requests", "expected_exact")
+    rc = lib().twe_request_confidence(C.byref(st), *[_ptr(x) for x in ins], *[_ptr(out[k]) for k in order])
+    return out, rc
+
+
+def _elementwise(name, v):
+    v = np.ascontiguousarray(v, np.float64)
+    got = np.zeros_like(v)
+    getattr(lib(), name)(C.c_int64(len(v)), _ptr(v), _ptr(got))
+    return got
+
+
+def conf_exp(d):
+    """tw_core.cuh's conf_exp of every element of d, on the CPU."""
+    return _elementwise("twe_conf_exp", d)
+
+
+def conf_log(x):
+    """tw_core.cuh's conf_log of every element of x, on the CPU."""
+    return _elementwise("twe_conf_log", x)

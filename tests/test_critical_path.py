@@ -6,53 +6,19 @@ overlapping, truncated and nested call; children that start before or end after 
 children; the callee-position tie; a callee inside and outside the batch; negative durations; a cycle; a
 detached fragment.  On synth.hotel_tree's truth every node is on the path and its self time has a closed form.
 On the trace directories of test_traces the self times of every request add up to its latency.  The CPU build
-of the device steps (tests/emul/tw_emul_critical.cpp) must give the host reference's arrays on all of them,
-with int64 times and with float64 times divided by 3 and 7."""
+of the device steps (tests/emul/tw_emul_critical.cpp, through emul_backend) must give the host reference's
+arrays on all of them, with int64 times and with float64 times divided by 3 and 7."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import emul_backend
 from traceweaver_b200 import _abi
-from traceweaver_b200.batch import HostBatch, Problem, batch_struct, build_batch
+from traceweaver_b200.batch import HostBatch, Problem, build_batch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 NODE_KEYS = ("root", "on_path", "self_us", "culprit")
 SUM_KEYS = ("server_us", "server_visits", "call_us", "requests")
-
-
-@pytest.fixture(scope="module")
-def emul(tmp_path_factory):
-    """The CPU build of the device steps (g++, as tests/emul/Makefile builds tw_emul.cpp)."""
-    so = str(tmp_path_factory.mktemp("emul") / "libtw_emul_critical.so")
-    subprocess.check_call([os.environ.get("CXX", "g++"), "-O2", "-fPIC", "-std=c++17", "-Wall", "-ffp-contract=off",
-                           "-shared", "-x", "c++", "-o", so, os.path.join(HERE, "emul", "tw_emul_critical.cpp"), "-lm"],
-                          stderr=subprocess.DEVNULL)
-    return C.CDLL(so)
-
-
-def emul_paths(lib, hb, assign, in_caller, root, slow_us, levels=0):
-    """The walk with the kernels' per-node steps, stepped on the CPU; the join's roots come in.  levels: the
-    level launches, the last of them walking what lies below it (cp_tail_walk); 0: until nothing is left."""
-    a = {k: np.ascontiguousarray(v) for k, v in hb.arrays.items()}
-    st = batch_struct(HostBatch(problems=hb.problems, arrays=a), lambda k: a[k].ctypes.data)
-    times = _abi.fill(_abi.TwTimesF64, a) if hb.float_times else None
-    n_in, n = int(hb.prob_in_off[-1]), int(hb.prob_in_off[-1]) + int(hb.ep_out_off[-1])
-    P, n_ep = hb.n_problems, int(hb.prob_ep_off[-1])
-    out = dict(on_path=np.zeros(n, np.uint8), self_us=np.zeros(n), culprit=np.zeros(n_in, np.int32),
-               server_us=np.zeros((P, 2)), server_visits=np.zeros((P, 2), np.int32), call_us=np.zeros((n_ep, 2)),
-               requests=np.zeros(2, np.int32))
-    links = [np.ascontiguousarray(x, np.int32).reshape(-1) for x in (assign, in_caller, root)]
-    ptr = lambda x: C.c_void_p(x.ctypes.data)
-    rc = lib.twe_critical_paths(C.byref(st), C.byref(times) if times is not None else None,
-                                *[ptr(x) for x in links], C.c_double(slow_us), C.c_int(levels),
-                                *[ptr(out[k]) for k in ("on_path", "self_us", "culprit", "server_us", "server_visits",
-                                                        "call_us", "requests")])
-    assert rc == 0
-    out["root"] = links[2]
-    return out
 
 
 def compressed(hb, cf):
@@ -91,17 +57,18 @@ def check_invariant(res, hb, exact):
     assert on[req].all()
 
 
-def paths_everywhere(emul, hb, assign, in_caller, slow_us=0.0):
+def paths_everywhere(hb, assign, in_caller, slow_us=0.0):
     """Host reference, with the invariant; the CPU step equal to it, int64 and float64 / 3, / 7."""
     from traceweaver_b200.traces import critical_paths_host
     want = critical_paths_host(hb, assign, in_caller, slow_us)
     check_invariant(want, hb, exact=True)
-    check_same(emul_paths(emul, hb, assign, in_caller, want["root"], slow_us), want, exact_sums=True)
+    check_same(emul_backend.critical_paths(hb, assign, in_caller, want["root"], slow_us), want, exact_sums=True)
     for cf in (3, 7):
         hf = compressed(hb, cf)
         wf = critical_paths_host(hf, assign, in_caller, slow_us / cf)
         check_invariant(wf, hf, exact=False)
-        check_same(emul_paths(emul, hf, assign, in_caller, wf["root"], slow_us / cf), wf, exact_sums=False)
+        check_same(emul_backend.critical_paths(hf, assign, in_caller, wf["root"], slow_us / cf), wf,
+                   exact_sums=False)
     return want
 
 
@@ -122,24 +89,24 @@ def _request(root, calls, callee=None):
     return build_batch(probs, validate=False), assign, in_caller
 
 
-def _walk(emul, root, calls, callee=None):
+def _walk(root, calls, callee=None):
     hb, assign, in_caller = _request(root, calls, callee)
-    res = paths_everywhere(emul, hb, assign, in_caller)
+    res = paths_everywhere(hb, assign, in_caller)
     n_in = int(hb.prob_in_off[-1])
     return res, n_in
 
 
-def test_sequential_calls_are_all_on_the_path(emul):
-    res, n_in = _walk(emul, (0, 100), [(10, 30), (40, 70), (75, 90)])
+def test_sequential_calls_are_all_on_the_path():
+    res, n_in = _walk((0, 100), [(10, 30), (40, 70), (75, 90)])
     assert res["on_path"].tolist() == [1, 1, 1, 1]
     assert res["self_us"].tolist() == [35.0, 20.0, 30.0, 15.0]
     assert res["culprit"].tolist() == [0]
     assert res["latency"].tolist() == [100.0]
 
 
-def test_parallel_calls_last_to_finish_truncated_and_nested(emul):
+def test_parallel_calls_last_to_finish_truncated_and_nested():
     # B ends last; A was still running when B started (truncated to [10, 20]); C lies inside B
-    res, _ = _walk(emul, (0, 100), [(10, 60), (20, 80), (30, 50)])
+    res, _ = _walk((0, 100), [(10, 60), (20, 80), (30, 50)])
     assert res["on_path"].tolist() == [1, 1, 1, 0]
     assert res["self_us"].tolist() == [30.0, 10.0, 60.0, 0.0]
     assert res["culprit"].tolist() == [2]
@@ -147,31 +114,31 @@ def test_parallel_calls_last_to_finish_truncated_and_nested(emul):
     assert res["call_us"].tolist() == [[10.0, 10.0], [60.0, 60.0], [0.0, 0.0]]
 
 
-def test_children_beyond_their_parent_are_clipped(emul):
-    res, _ = _walk(emul, (0, 100), [(-10, 50), (60, 120)])
+def test_children_beyond_their_parent_are_clipped():
+    res, _ = _walk((0, 100), [(-10, 50), (60, 120)])
     assert res["self_us"].tolist() == [10.0, 50.0, 40.0]
 
 
-def test_zero_length_and_outside_children_are_off_the_path(emul):
-    res, _ = _walk(emul, (0, 100), [(50, 50), (150, 160), (20, 30)])
+def test_zero_length_and_outside_children_are_off_the_path():
+    res, _ = _walk((0, 100), [(50, 50), (150, 160), (20, 30)])
     assert res["on_path"].tolist() == [1, 0, 0, 1]
     assert res["self_us"].tolist() == [90.0, 0.0, 0.0, 10.0]
 
 
-def test_callee_position_breaks_a_tie(emul):
+def test_callee_position_breaks_a_tie():
     # both end at 80: callee 0 first; callee 1 was running when it started and is truncated to [20, 40]
-    res, _ = _walk(emul, (0, 100), [(40, 80), (20, 80)])
+    res, _ = _walk((0, 100), [(40, 80), (20, 80)])
     assert res["on_path"].tolist() == [1, 1, 1]
     assert res["self_us"].tolist() == [40.0, 40.0, 20.0]
     # callee 0 first again; callee 1 starts after it and is nested
-    res, _ = _walk(emul, (0, 100), [(20, 80), (40, 80)])
+    res, _ = _walk((0, 100), [(20, 80), (40, 80)])
     assert res["on_path"].tolist() == [1, 1, 0]
     assert res["self_us"].tolist() == [40.0, 60.0, 0.0]
 
 
-def test_callee_inside_and_outside_the_batch(emul):
+def test_callee_inside_and_outside_the_batch():
     # call 0's server span is in the batch (clipped to the call), call 1's is not: all of it is call time
-    res, n_in = _walk(emul, (0, 100), [(10, 30), (40, 90)], callee=(5, 25))
+    res, n_in = _walk((0, 100), [(10, 30), (40, 90)], callee=(5, 25))
     assert n_in == 2
     # nodes: in 0 (root), in 1 (callee), out 2 (call 0), out 3 (call 1), out 4 (the callee's unmade call)
     assert res["on_path"].tolist() == [1, 1, 1, 1, 0]
@@ -181,48 +148,48 @@ def test_callee_inside_and_outside_the_batch(emul):
     assert res["server_visits"].tolist() == [[1, 1], [1, 1]]
 
 
-def test_negative_durations_are_empty(emul):
-    res, _ = _walk(emul, (100, 40), [(50, 60)])              # a root that ends before it starts
+def test_negative_durations_are_empty():
+    res, _ = _walk((100, 40), [(50, 60)])              # a root that ends before it starts
     assert res["on_path"].tolist() == [1, 0]
     assert res["self_us"].tolist() == [0.0, 0.0]
     assert res["latency"].tolist() == [0.0]
-    res, _ = _walk(emul, (0, 100), [(60, 40), (10, 20)])      # a call that ends before it starts
+    res, _ = _walk((0, 100), [(60, 40), (10, 20)])      # a call that ends before it starts
     assert res["on_path"].tolist() == [1, 0, 1]
     assert res["self_us"].tolist() == [90.0, 0.0, 10.0]
 
 
-def test_cycle_and_detached_fragment_belong_to_no_request(emul):
+def test_cycle_and_detached_fragment_belong_to_no_request():
     from test_traces import _two_in_spans
     hb = _two_in_spans()                                 # in 0 [100, 150], in 1 [200, 250]; out 2, 3
-    res = paths_everywhere(emul, hb, [0, 1], [2, -1])    # in 0 and out 2 form a cycle
+    res = paths_everywhere(hb, [0, 1], [2, -1])    # in 0 and out 2 form a cycle
     assert res["root"].tolist() == [-1, 1, -1, 1]
     assert res["on_path"].tolist() == [0, 1, 0, 1]
     assert res["self_us"].tolist() == [0.0, 40.0, 0.0, 10.0]
     assert res["culprit"].tolist() == [-1, 1]
     assert res["requests"].tolist() == [1, 1]
-    res = paths_everywhere(emul, hb, [0, -1], [-1, -1])  # out 3 is a detached fragment
+    res = paths_everywhere(hb, [0, -1], [-1, -1])  # out 3 is a detached fragment
     assert res["on_path"].tolist() == [1, 1, 1, 0]
     assert res["requests"].tolist() == [2, 2]
 
 
-def test_slow_column_takes_the_requests_at_or_above_the_threshold(emul):
+def test_slow_column_takes_the_requests_at_or_above_the_threshold():
     from traceweaver_b200 import synth
     from traceweaver_b200.traces import critical_paths_host
     tree = synth.hotel_tree(2, 60, 120.0, seed=3)
     hb = tree["hb"]
     lat = critical_paths_host(hb, tree["truth"], tree["in_caller"], 0.0)["latency"]
     thr = float(np.sort(lat)[int(0.9 * (len(lat) - 1))])
-    res = paths_everywhere(emul, hb, tree["truth"], tree["in_caller"], thr)
+    res = paths_everywhere(hb, tree["truth"], tree["in_caller"], thr)
     assert res["requests"].tolist() == [len(lat), int((lat >= thr).sum())]
     assert (res["server_visits"][:, 1] <= res["server_visits"][:, 0]).all()
     assert res["server_visits"][:, 1].sum() == 2 * int((lat >= thr).sum())
 
 
-def test_generated_truth_puts_every_node_on_the_path(emul):
+def test_generated_truth_puts_every_node_on_the_path():
     from traceweaver_b200 import synth
     tree = synth.hotel_tree(3, 200, 150.0, seed=2)
     hb = tree["hb"]
-    res = paths_everywhere(emul, hb, tree["truth"], tree["in_caller"])
+    res = paths_everywhere(hb, tree["truth"], tree["in_caller"])
     assert (res["on_path"] == 1).all()
     # closed form: the generator's calls are sequential and inside their caller, every server span inside
     # its client span, so a node's self time is its length less its children's
@@ -241,11 +208,11 @@ def test_generated_truth_puts_every_node_on_the_path(emul):
 
 
 @pytest.mark.parametrize("layout", ["hotel", "node", "alibaba"])
-def test_self_times_add_up_on_trace_directories(emul, tmp_path, layout):
+def test_self_times_add_up_on_trace_directories(tmp_path, layout):
     from test_traces import ALIBABA_DIR, _tree_dir, load_batch
     directory = ALIBABA_DIR if layout == "alibaba" else _tree_dir(tmp_path, layout)
     services, hb, in_caller, truth, tid = load_batch(directory, layout)
-    res = paths_everywhere(emul, hb, truth, in_caller)
+    res = paths_everywhere(hb, truth, in_caller)
     assert res["requests"][0] == len(np.unique(tid))
 
 

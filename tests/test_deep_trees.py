@@ -13,12 +13,13 @@ import numpy as np
 import pytest
 
 from deep_tree_util import ORDERS, TIMINGS, deep_trees
-from test_critical_path import check_invariant, check_same, compressed, emul, emul_paths  # noqa: F401
+import emul_backend
+from test_critical_path import check_invariant, check_same, compressed
 
 LEVELS = range(1, 65)
 
 
-def _sweep(emul, g, levels=LEVELS):
+def _sweep(g, levels=LEVELS):
     """Host reference with the invariant; the CPU step equal to it at every level count, int64 and
     float64 / 3, / 7."""
     from traceweaver_b200.traces import critical_paths_host
@@ -29,37 +30,37 @@ def _sweep(emul, g, levels=LEVELS):
         want = critical_paths_host(h, assign, in_caller, 0.0)
         check_invariant(want, h, exact=cf is None)
         for L in (0, *levels):
-            got = emul_paths(emul, h, assign, in_caller, want["root"], 0.0, levels=L)
+            got = emul_backend.critical_paths(h, assign, in_caller, want["root"], 0.0, levels=L)
             check_same(got, want, exact_sums=cf is None)
         res.append(want)
     return res[0]
 
 
 @pytest.mark.parametrize("spine", ["first", "last"])
-def test_tail_walk_gives_the_same_paths_at_every_level_count(emul, spine):
+def test_tail_walk_gives_the_same_paths_at_every_level_count(spine):
     g = deep_trees(20, callees=8, spine=spine, requests=3, seed=5)
-    res = _sweep(emul, g)
+    res = _sweep(g)
     assert (res["on_path"] == 1).all()
 
 
 @pytest.mark.parametrize("spine", ["first", "last"])
-def test_tail_walk_on_every_call_timing(emul, spine):
+def test_tail_walk_on_every_call_timing(spine):
     for q, timing in enumerate(TIMINGS + ("mixed",)):
-        _sweep(emul, deep_trees(12, callees=5, spine=spine, timing=timing, requests=2, order=ORDERS[q % 3],
-                                seed=10 + q))
+        _sweep(deep_trees(12, callees=5, spine=spine, timing=timing, requests=2, order=ORDERS[q % 3],
+                          seed=10 + q))
 
 
 @pytest.mark.parametrize("order", ORDERS)
-def test_tail_walk_on_random_shapes(emul, order):
+def test_tail_walk_on_random_shapes(order):
     g = deep_trees(16, callees=8, random_shape=True, requests=12, timing="mixed", order=order, seed=21)
     assert (g["depth"] > 1).any() and (g["assign"] == -1).any()
-    _sweep(emul, g)
+    _sweep(g)
 
 
-def test_tail_walk_below_level_1_of_a_deep_tree(emul):
+def test_tail_walk_below_level_1_of_a_deep_tree():
     # 600 levels of spine-last calls: the first level's threads walk all of it
     g = deep_trees(600, callees=3, spine="last", requests=2, seed=7)
-    res = _sweep(emul, g, levels=(1, 2, 33, 64))
+    res = _sweep(g, levels=(1, 2, 33, 64))
     assert (res["on_path"] == 1).all()
 
 
@@ -75,12 +76,12 @@ def test_self_times_add_up_on_generated_trees(timing, order):
 
 
 @pytest.mark.parametrize("callees", [1, 2, 8])
-def test_sequential_spine_first_trees_have_the_closed_form(emul, callees):
+def test_sequential_spine_first_trees_have_the_closed_form(callees):
     from traceweaver_b200.traces import parents_host
     g = deep_trees(30, callees=callees, spine="first", timing="sequential", requests=3, order="shuffled",
                    seed=callees)
     hb = g["hb"]
-    res = _sweep(emul, g, levels=(1, 3, 64))
+    res = _sweep(g, levels=(1, 3, 64))
     assert (res["on_path"] == 1).all()
     # the calls are sequential and inside their caller, every server span inside its client span: a node's
     # self time is its length less its children's
@@ -94,9 +95,9 @@ def test_sequential_spine_first_trees_have_the_closed_form(emul, callees):
     assert sorted(np.flatnonzero(res["culprit"] >= 0).tolist()) == sorted(g["roots"].tolist())
 
 
-def test_equal_self_times_pick_the_smallest_node(emul):
+def test_equal_self_times_pick_the_smallest_node():
     g = deep_trees(50, callees=4, spine="last", requests=3, order="shuffled", const_times=True, seed=3)
-    res = _sweep(emul, g, levels=(1, 7, 64))
+    res = _sweep(g, levels=(1, 7, 64))
     on, self_us, root = res["on_path"] == 1, res["self_us"], res["root"]
     for r in g["roots"]:
         mine = np.flatnonzero(on & (root == r))

@@ -5,7 +5,8 @@ wrong sizes; run-to-run identity; solve() untouched by a later request_confidenc
 import numpy as np
 import pytest
 
-from test_request_confidence import KEYS, check_same, emul, emul_confidence  # noqa: F401  (emul: a fixture)
+import emul_backend
+from test_request_confidence import KEYS, check_same
 
 pytestmark = pytest.mark.gpu
 DEV_KEYS = tuple(k for k in KEYS if k != "q")
@@ -33,7 +34,7 @@ def _truth_out(solver, hb, truth, out):
                 topk_score=out["topk_score"], topk_idx=out["topk_idx"], topk_cnt=out["topk_cnt"])
 
 
-def _same_everywhere(solver, emul, hb, out, in_caller):
+def _same_everywhere(solver, hb, out, in_caller):
     from traceweaver_b200.traces import request_confidence_host
     got = solver.request_confidence(hb, out, in_caller)
     topk = {k: out[k] for k in ("topk_score", "topk_idx", "topk_cnt")}
@@ -42,8 +43,8 @@ def _same_everywhere(solver, emul, hb, out, in_caller):
                       expected_exact=np.array([got["expected_exact"]]))
     check_same(got_arrays, want, keys=DEV_KEYS + ("root",))
     n_in = int(hb.prob_in_off[-1])
-    cpu, rc = emul_confidence(emul, hb, out["assign"], got["root"][:n_in], out["chosen_score"], out["chosen_code"],
-                              topk)
+    cpu, rc = emul_backend.request_confidence(hb, out["assign"], got["root"][:n_in], out["chosen_score"],
+                                              out["chosen_code"], topk)
     assert rc == 0
     check_same(got_arrays, cpu, keys=DEV_KEYS)
     asm = solver.assemble(hb, out["assign"], in_caller)
@@ -59,34 +60,34 @@ def _same_everywhere(solver, emul, hb, out, in_caller):
 
 
 @pytest.mark.parametrize("layout", ["hotel", "node", "alibaba"])
-def test_device_equals_host_on_trace_directories(solver, emul, tmp_path, layout):  # noqa: F811
+def test_device_equals_host_on_trace_directories(solver, tmp_path, layout):
     from test_traces import ALIBABA_DIR, _tree_dir, load_batch
     directory = ALIBABA_DIR if layout == "alibaba" else _tree_dir(tmp_path, layout, n_req=300)
     _, hb, in_caller, truth, _ = load_batch(directory, layout)
     out = _solved(solver, hb)
-    _same_everywhere(solver, emul, hb, out, in_caller)
-    _same_everywhere(solver, emul, hb, _truth_out(solver, hb, truth, out), in_caller)
+    _same_everywhere(solver, hb, out, in_caller)
+    _same_everywhere(solver, hb, _truth_out(solver, hb, truth, out), in_caller)
 
 
-def test_device_equals_host_on_a_batch_solve_splits(solver, emul):  # noqa: F811
+def test_device_equals_host_on_a_batch_solve_splits(solver):
     from traceweaver_b200 import synth
     tree = synth.hotel_tree(560, 1000, 100.0, seed=31)
     hb = tree["hb"]
     assert int(hb.prob_in_off[-1]) > 1 << 20
     out = _solved(solver, hb)
     assert solver.last_chunks > 1
-    got = _same_everywhere(solver, emul, hb, out, tree["in_caller"])
+    got = _same_everywhere(solver, hb, out, tree["in_caller"])
     assert got["requests"] == 560 * 1000
-    _same_everywhere(solver, emul, hb, _truth_out(solver, hb, tree["truth"], out), tree["in_caller"])
+    _same_everywhere(solver, hb, _truth_out(solver, hb, tree["truth"], out), tree["in_caller"])
 
 
-def test_device_equals_host_on_float64_times(solver, emul):  # noqa: F811
+def test_device_equals_host_on_float64_times(solver):
     from test_critical_path import compressed
     from traceweaver_b200 import synth
     tree = synth.hotel_tree(4, 300, 120.0, seed=8)
     hf = compressed(tree["hb"], 7)
     assert hf.float_times
-    _same_everywhere(solver, emul, hf, _solved(solver, hf), tree["in_caller"])
+    _same_everywhere(solver, hf, _solved(solver, hf), tree["in_caller"])
 
 
 def test_two_calls_are_byte_identical(solver):

@@ -5,54 +5,20 @@ Hand-built batches check each rule of the definition in traces.py: a single cand
 rank 0, at a later rank and not listed; a duplicate of the chosen tuple in the list; the NA and infeasible
 codes; a request with a zero decision; exp underflow; the weakest decision's tie; a detached fragment; a
 cycle.  Deep chains from deep_tree_util and random inputs cover the per-request sums.  The CPU build of the
-device step (tests/emul/tw_emul_confidence.cpp) must give the host restatement's arrays bit for bit on all
-of them and on the final top-K rows of every golden service.  On the pooled golden services the share of
-right in-spans must rise strictly over bins of p."""
-import ctypes as C
+device step (tests/emul/tw_emul_confidence.cpp, through emul_backend) must give the host restatement's arrays
+bit for bit on all of them and on the final top-K rows of every golden service.  On the pooled golden services
+the share of right in-spans must rise strictly over bins of p."""
 import math
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+import emul_backend
 from traceweaver_b200 import _abi
-from traceweaver_b200.batch import HostBatch, batch_struct
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 K = _abi.TW_K
 KEYS = ("p", "ell", "decisions", "zero", "log_conf", "conf", "weakest", "weakest_p", "est_accuracy", "requests",
         "expected_exact", "q")
-
-
-@pytest.fixture(scope="module")
-def emul(tmp_path_factory):
-    """The CPU build of the device step (g++, as tests/emul/Makefile builds tw_emul.cpp)."""
-    so = str(tmp_path_factory.mktemp("emul") / "libtw_emul_confidence.so")
-    subprocess.check_call([os.environ.get("CXX", "g++"), "-O2", "-fPIC", "-std=c++17", "-Wall", "-ffp-contract=off",
-                           "-shared", "-x", "c++", "-o", so, os.path.join(HERE, "emul", "tw_emul_confidence.cpp"),
-                           "-lm"], stderr=subprocess.DEVNULL)
-    return C.CDLL(so)
-
-
-def emul_confidence(lib, hb, assign, root, score, code, topk):
-    """The step, the per-request passes and the fixed-order sums of tw_confidence.cu stepped on the CPU; the
-    join's roots come in.  Returns the arrays and the return code."""
-    a = {k: np.ascontiguousarray(v) for k, v in hb.arrays.items()}
-    st = batch_struct(HostBatch(problems=hb.problems, arrays=a), lambda k: a[k].ctypes.data)
-    n_in, P = int(hb.prob_in_off[-1]), hb.n_problems
-    ins = [np.ascontiguousarray(np.asarray(x, t).reshape(-1)) for x, t in
-           ((assign, np.int32), (root, np.int32), (score, np.float64), (code, np.uint8),
-            (topk["topk_score"], np.float64), (topk["topk_idx"], np.int32), (topk["topk_cnt"], np.uint8))]
-    out = dict(p=np.zeros(n_in), ell=np.zeros(n_in), q=np.zeros(n_in, np.int64), decisions=np.zeros(n_in, np.int32),
-               zero=np.zeros(n_in, np.int32), log_conf=np.zeros(n_in, np.int64), conf=np.zeros(n_in),
-               weakest=np.zeros(n_in, np.int32), weakest_p=np.zeros(n_in), est_accuracy=np.zeros(P),
-               requests=np.zeros(1, np.int32), expected_exact=np.zeros(1))
-    ptr = lambda x: C.c_void_p(x.ctypes.data)
-    order = ("p", "ell", "q", "decisions", "zero", "log_conf", "conf", "weakest", "weakest_p", "est_accuracy",
-             "requests", "expected_exact")
-    rc = lib.twe_request_confidence(C.byref(st), *[ptr(x) for x in ins], *[ptr(out[k]) for k in order])
-    return out, rc
 
 
 def check_same(got, want, keys=KEYS):
@@ -61,11 +27,11 @@ def check_same(got, want, keys=KEYS):
         assert g.tobytes() == w.astype(g.dtype).tobytes(), k
 
 
-def everywhere(emul, hb, assign, in_caller, score, code, topk):
+def everywhere(hb, assign, in_caller, score, code, topk):
     """The host restatement, and the CPU step equal to it bit for bit."""
     from traceweaver_b200.traces import request_confidence_host
     want = request_confidence_host(hb, assign, in_caller, score, code, topk)
-    got, rc = emul_confidence(emul, hb, assign, want["root"][:int(hb.prob_in_off[-1])], score, code, topk)
+    got, rc = emul_backend.request_confidence(hb, assign, want["root"][:int(hb.prob_in_off[-1])], score, code, topk)
     assert rc == 0
     check_same(got, want)
     n_in = int(hb.prob_in_off[-1])
@@ -106,59 +72,59 @@ def _inputs(rows, scores, codes):
                                                                               topk_cnt=cnt)
 
 
-def _one(emul, row_a, score_a, code_a=0, row_b=((-1.0, 0),), score_b=-1.0, code_b=0, links="request"):
+def _one(row_a, score_a, code_a=0, row_b=((-1.0, 0),), score_b=-1.0, code_b=0, links="request"):
     hb, assign, in_caller = _pair(links)
     score, code, topk = _inputs([row_a, row_b], [score_a, score_b], [code_a, code_b])
-    return everywhere(emul, hb, assign, in_caller, score, code, topk)
+    return everywhere(hb, assign, in_caller, score, code, topk)
 
 
 def _share(sc, others):
     return math.exp(sc) / (math.exp(sc) + sum(math.exp(s) for s in others))
 
 
-def test_single_candidate_is_certain(emul):
-    res = _one(emul, [(-3.0, 0)], -3.0)
+def test_single_candidate_is_certain():
+    res = _one([(-3.0, 0)], -3.0)
     assert res["p"][0] == 1.0 and res["ell"][0] == 0.0 and res["q"][0] == 0
     assert res["conf"][0] == 1.0 and res["requests"][0] == 1 and res["decisions"].tolist() == [2, 0]
 
 
-def test_chosen_at_rank_zero_and_at_a_later_rank(emul):
-    res = _one(emul, [(-1.0, 0), (-2.0, 1), (-3.0, 2)], -1.0)
+def test_chosen_at_rank_zero_and_at_a_later_rank():
+    res = _one([(-1.0, 0), (-2.0, 1), (-3.0, 2)], -1.0)
     assert res["p"][0] == pytest.approx(_share(-1.0, [-2.0, -3.0]), rel=1e-15)
     assert res["ell"][0] == pytest.approx(-math.log(_share(-1.0, [-2.0, -3.0])), rel=1e-15)
-    res = _one(emul, [(-1.0, 1), (-2.0, 0), (-3.0, 2)], -2.0)
+    res = _one([(-1.0, 1), (-2.0, 0), (-3.0, 2)], -2.0)
     assert res["p"][0] == pytest.approx(_share(-2.0, [-1.0, -3.0]), rel=1e-15)
 
 
-def test_chosen_not_listed_counts_with_its_own_score(emul):
-    res = _one(emul, [(-1.0, 1), (-2.0, 2)], -5.0)
+def test_chosen_not_listed_counts_with_its_own_score():
+    res = _one([(-1.0, 1), (-2.0, 2)], -5.0)
     assert res["p"][0] == pytest.approx(_share(-5.0, [-1.0, -2.0]), rel=1e-14)
 
 
-def test_a_duplicate_of_the_chosen_tuple_is_not_an_alternative(emul):
-    res = _one(emul, [(-1.0, 0), (-2.0, 1), (-1.0, 0)], -1.0)
+def test_a_duplicate_of_the_chosen_tuple_is_not_an_alternative():
+    res = _one([(-1.0, 0), (-2.0, 1), (-1.0, 0)], -1.0)
     assert res["p"][0] == pytest.approx(_share(-1.0, [-2.0]), rel=1e-15)
 
 
 @pytest.mark.parametrize("code", [_abi.TW_ASSESS_NA, _abi.TW_ASSESS_RANGE, _abi.TW_ASSESS_CONTAIN,
                                   _abi.TW_ASSESS_ORDER])
-def test_unscored_choice_is_a_zero_decision(emul, code):
-    res = _one(emul, [(-1.0, 1)], np.nan, code_a=code, row_b=[(-1.0, 0), (-2.0, 1)], score_b=-1.0)
+def test_unscored_choice_is_a_zero_decision(code):
+    res = _one([(-1.0, 1)], np.nan, code_a=code, row_b=[(-1.0, 0), (-2.0, 1)], score_b=-1.0)
     assert res["p"][0] == 0.0 and res["ell"][0] == np.inf and res["q"][0] == -1
     assert res["zero"][0] == 1 and res["conf"][0] == 0.0
     assert res["log_conf"][0] == res["q"][1] > 0                       # the other decision still adds up
     assert res["weakest"][0] == 0 and res["weakest_p"][0] == 0.0
 
 
-def test_exp_underflow_is_a_zero_decision(emul):
-    res = _one(emul, [(-1.0, 1)], -1000.0)
+def test_exp_underflow_is_a_zero_decision():
+    res = _one([(-1.0, 1)], -1000.0)
     assert res["p"][0] == 0.0 and res["ell"][0] == np.inf and res["zero"][0] == 1
-    res = _one(emul, [(-1.0, 1)], -700.0)                              # tiny but not zero
+    res = _one([(-1.0, 1)], -700.0)                              # tiny but not zero
     assert 0.0 < res["p"][0] < 1e-300 and res["ell"][0] == pytest.approx(699.0, rel=1e-12)
 
 
-def test_request_sums_and_weakest(emul):
-    res = _one(emul, [(-1.0, 0), (-2.0, 1)], -1.0, row_b=[(-1.0, 1), (-1.5, 0)], score_b=-1.5)
+def test_request_sums_and_weakest():
+    res = _one([(-1.0, 0), (-2.0, 1)], -1.0, row_b=[(-1.0, 1), (-1.5, 0)], score_b=-1.5)
     pa, pb = _share(-1.0, [-2.0]), _share(-1.5, [-1.0])
     assert res["weakest"][0] == 1 and res["weakest_p"][0] == res["p"][1]
     assert res["log_conf"][0] == res["q"][0] + res["q"][1]
@@ -168,19 +134,19 @@ def test_request_sums_and_weakest(emul):
     assert np.isnan(res["conf"][1]) and res["weakest"][1] == -1
 
 
-def test_weakest_tie_takes_the_smallest_node(emul):
-    res = _one(emul, [(-1.0, 0), (-2.0, 1)], -1.0, row_b=[(-1.0, 0), (-2.0, 1)], score_b=-1.0)
+def test_weakest_tie_takes_the_smallest_node():
+    res = _one([(-1.0, 0), (-2.0, 1)], -1.0, row_b=[(-1.0, 0), (-2.0, 1)], score_b=-1.0)
     assert res["p"][0] == res["p"][1] and res["weakest"][0] == 0
 
 
-def test_detached_fragment_and_cycle_belong_to_no_request(emul):
-    res = _one(emul, [(-1.0, 0)], -1.0, links="detached")                # B's caller was taken by no in-span
+def test_detached_fragment_and_cycle_belong_to_no_request():
+    res = _one([(-1.0, 0)], -1.0, links="detached")                # B's caller was taken by no in-span
     assert res["root"][:2].tolist() == [0, 2] and res["decisions"].tolist() == [1, 0]
     assert res["requests"][0] == 1 and np.isnan(res["conf"][1])
-    res = _one(emul, [(-1.0, 0)], -1.0, links="cycle")
+    res = _one([(-1.0, 0)], -1.0, links="cycle")
     assert res["root"].tolist() == [-1] * 4 and res["requests"][0] == 0 and res["decisions"].tolist() == [0, 0]
     assert res["expected_exact"][0] == 0.0 and res["p"][0] == 1.0
-    res = _one(emul, [(-1.0, 0)], -1.0, links="apart")
+    res = _one([(-1.0, 0)], -1.0, links="apart")
     assert res["requests"][0] == 2 and res["expected_exact"][0] == res["conf"][0] + res["conf"][1]
 
 
@@ -231,33 +197,32 @@ def random_inputs(hb, assign, seed):
 
 
 @pytest.mark.parametrize("depth,spine,seed", [(12, "last", 1), (20, "first", 2), (40, "last", 3)])
-def test_deep_chains(emul, depth, spine, seed):
+def test_deep_chains(depth, spine, seed):
     from deep_tree_util import deep_trees
     t = deep_trees(depth, callees=3, spine=spine, requests=3, random_shape=True, order="shuffled", seed=seed)
     score, code, topk = random_inputs(t["hb"], t["assign"], seed)
-    res = everywhere(emul, t["hb"], t["assign"], t["in_caller"], score, code, topk)
+    res = everywhere(t["hb"], t["assign"], t["in_caller"], score, code, topk)
     assert sorted(np.flatnonzero(res["root"][:len(res["p"])] == np.arange(len(res["p"])))) == sorted(t["roots"])
     assert res["requests"][0] == 3
 
 
-def test_trace_directories(emul, tmp_path):
+def test_trace_directories(tmp_path):
     from test_traces import ALIBABA_DIR, _tree_dir, load_batch
     for layout in ("hotel", "node", "alibaba"):
         directory = ALIBABA_DIR if layout == "alibaba" else _tree_dir(tmp_path, layout, n_req=120)
         _, hb, in_caller, truth, _ = load_batch(directory, layout)
         score, code, topk = random_inputs(hb, truth, 7)
-        everywhere(emul, hb, truth, in_caller, score, code, topk)
+        everywhere(hb, truth, in_caller, score, code, topk)
 
 
-def test_exp_and_log_are_the_same_on_both_builds(emul):
+def test_exp_and_log_are_the_same_on_both_builds():
     from traceweaver_b200.traces import conf_exp, conf_log
     rng = np.random.default_rng(0)
     d = -np.concatenate([np.linspace(0.0, 750.0, 30001), rng.exponential(5.0, 30000), [0.0, 745.5, np.inf]])
     x = np.concatenate([1.0 + rng.random(30000) * 5.0, np.exp(np.linspace(-700, 700, 20001)), [1.0, 6.0]])
-    for f, name, v in ((conf_exp, "twe_conf_exp", d), (conf_log, "twe_conf_log", x)):
-        got = np.zeros_like(v)
-        getattr(emul, name)(C.c_int64(len(v)), C.c_void_p(v.ctypes.data), C.c_void_p(got.ctypes.data))
-        assert got.tobytes() == f(v).tobytes(), name
+    for f, cpu, v in ((conf_exp, emul_backend.conf_exp, d), (conf_log, emul_backend.conf_log, x)):
+        got = cpu(v)
+        assert got.tobytes() == f(v).tobytes(), f.__name__
     ref = np.exp(d[d > -708])
     assert np.max(np.abs(conf_exp(d[d > -708]) - ref) / ref) < 3e-16
     assert np.max(np.abs(conf_log(x) - np.log(x)) / np.maximum(np.abs(np.log(x)), 1e-300)) < 4e-16
@@ -270,7 +235,7 @@ def test_exp_and_log_are_the_same_on_both_builds(emul):
 BINS = (0.0, 0.5, 0.8, 0.95, 0.99, 0.999, 1.0 + 1e-12)
 
 
-def golden_choices(emul):
+def golden_choices():
     from golden_util import Golden, golden_files
     from oracle.tw_oracle import OracleBatch
     from traceweaver_b200.batch import build_batch
@@ -290,7 +255,7 @@ def golden_choices(emul):
         at = np.where(listed.any(axis=1), listed.argmax(axis=1), -1)
         score[at >= 0] = top["topk_score"][at >= 0, at[at >= 0]]          # the listed score where it is listed
         p, ell, q = choice_host(hb, a, score, sc["code"], top)
-        got, rc = emul_confidence(emul, hb, a, np.arange(n, dtype=np.int32), score, sc["code"], top)
+        got, rc = emul_backend.request_confidence(hb, a, np.arange(n, dtype=np.int32), score, sc["code"], top)
         assert rc == 0
         check_same(got, dict(p=p, ell=ell, q=q), keys=("p", "ell", "q"))
         ps.append(p)
@@ -298,8 +263,8 @@ def golden_choices(emul):
     return np.concatenate(ps), np.concatenate(right)
 
 
-def test_golden_services_rank_right_choices_higher(emul):
-    p, right = golden_choices(emul)
+def test_golden_services_rank_right_choices_higher():
+    p, right = golden_choices()
     b = np.digitize(p, BINS) - 1
     share = [right[b == k].mean() for k in range(len(BINS) - 1)]
     assert all((b == k).sum() > 100 for k in range(len(BINS) - 1))

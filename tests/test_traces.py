@@ -198,3 +198,25 @@ def test_generated_tree_joins_to_requests():
     assert (root >= 0).all() and (root < 600).all()        # every node under a frontend in-span
     assert (size[:600] == 7).all()
     assert np.array_equal(tree["in_request"][root[:n_in]], tree["in_request"])
+
+
+@pytest.mark.gpu
+def test_device_join_converts_int64_links():
+    """traces.assemble reads int64 assign / in_caller tensors as the int32 ones: the same join."""
+    import torch
+    if not torch.cuda.is_available():
+        pytest.fail("gpu-marked test needs a CUDA device")
+    from traceweaver_b200 import synth, traces
+    from traceweaver_b200.api import BatchSolver
+    tree = synth.hotel_tree(3, 200, 150.0, seed=2)
+    solver = BatchSolver(device=0, seed_select=10)
+    try:
+        eng = solver.engine
+        assign = torch.from_numpy(np.asarray(tree["truth"], np.int32)).to(eng.device)
+        in_caller = torch.from_numpy(np.asarray(tree["in_caller"], np.int32)).to(eng.device)
+        want = traces.assemble(eng, tree["hb"], assign, in_caller)
+        got = traces.assemble(eng, tree["hb"], assign.long(), in_caller.long())
+        for k in ("parent", "root", "size"):
+            assert torch.equal(got[k], want[k]), k
+    finally:
+        solver.close()

@@ -254,7 +254,7 @@ class BatchSolver:
         nodes it holds under the truth; -1 for an in-span that is not a root."""
         from . import traces
         eng = self.engine
-        links = _to_device(dict(in_caller=np.asarray(in_caller, np.int32).reshape(-1)), eng.device)["in_caller"]
+        links = traces.upload_inputs(eng, hb, "assemble", in_caller=in_caller)["in_caller"]
         res = traces.assemble(eng, hb, assign, links)
         out = {k: v.cpu().numpy() for k, v in res.items()}
         if truth is not None:
@@ -273,7 +273,7 @@ class BatchSolver:
         from . import traces
         eng = self.engine
         spans = traces.upload_spans(eng, hb)
-        links = _to_device(dict(in_caller=np.asarray(in_caller, np.int32).reshape(-1)), eng.device)["in_caller"]
+        links = traces.upload_inputs(eng, hb, "critical_paths", in_caller=in_caller)["in_caller"]
         req, lat = traces.request_latencies(spans, links)
         slow_us = traces.lower_quantile(lat, slow_quantile)
         res = traces.critical_paths(eng, hb, assign, links, slow_us, spans=spans)

@@ -97,17 +97,16 @@ struct tw_engine {
   DevBuf<int> order_missing;
   DevBuf<uint8_t> acc_flags;
   DevBuf<unsigned long long> acc_first;
-  // request trees (tw_assemble_traces): caller claim words, error words + per-round flags, and what the
-  // last call did (tw_debug_trace_rounds)
+  // request trees (tw_assemble_traces): caller claim words, error words + per-round flags, the parent and
+  // size words of a join whose caller keeps only the roots (tw_critical_paths, tw_request_confidence), and
+  // what the last call did (tw_debug_trace_rounds)
   DevBuf<int32_t> trace_claim;
   DevBuf<int32_t> trace_flags;
+  DevBuf<int32_t> trace_parent;
+  DevBuf<int32_t> trace_size;
   int trace_rounds_launched = 0, trace_rounds_run = 0, trace_still = 0;
-  // critical paths (tw_critical_paths): the join's parent and size words (tw_request_confidence's too), the
-  // walk's scratch (CpScratch),
-  // the level launches of the last call (tw_debug_critical_levels) and a forced level count, 0 = from the
-  // rounds (tw_debug_critical_force_levels)
-  DevBuf<int32_t> cp_parent;
-  DevBuf<int32_t> cp_size;
+  // critical paths (tw_critical_paths): the walk's scratch (CpScratch), the level launches of the last call
+  // (tw_debug_critical_levels) and a forced level count, 0 = from the rounds (tw_debug_critical_force_levels)
   DevBuf<int32_t> cp_level;
   DevBuf<int64_t> cp_wlo;
   DevBuf<int64_t> cp_whi;
@@ -726,12 +725,21 @@ static int trace_check(const tw_batch* h, const char* who) {
 }
 
 // The join of tw_assemble_traces after trace_check: its launches, the read-back of its error words and
-// round flags, and its errors (named after `who`).  Leaves the caller-claim words in eng->trace_claim.
+// round flags, and its errors (named after `who`).  A NULL parent_out / size_out goes to the engine's
+// eng->trace_parent / eng->trace_size.  Leaves the caller-claim words in eng->trace_claim.
 static int trace_join(tw_engine* eng, const tw_batch* dev, const tw_batch* h, const int32_t* assign,
                       const int32_t* in_caller, int32_t* parent_out, int32_t* root_out, int32_t* size_out,
                       const char* who, cudaStream_t s) {
   const int64_t n_in = h->n_in_total, n_out = h->n_out_total, n_nodes = n_in + n_out;
   const int rounds = trace_rounds(n_nodes);
+  if (!parent_out) {
+    CU(eng->trace_parent.reserve((size_t)n_nodes));
+    parent_out = eng->trace_parent.p;
+  }
+  if (!size_out) {
+    CU(eng->trace_size.reserve((size_t)n_nodes));
+    size_out = eng->trace_size.p;
+  }
   CU(eng->trace_claim.reserve((size_t)n_out));
   CU(eng->trace_flags.reserve((size_t)(4 + rounds)));
   int32_t* err = eng->trace_flags.p;
@@ -783,16 +791,14 @@ int tw_critical_paths(tw_engine* eng, const tw_batch* dev, const tw_batch* h, co
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream_;
   CU(cudaSetDevice(eng->device));
-  const int64_t n_in = h->n_in_total, n_nodes = n_in + h->n_out_total;
-  CU(eng->cp_parent.reserve((size_t)n_nodes));
-  CU(eng->cp_size.reserve((size_t)n_nodes));
+  const int64_t n_in = h->n_in_total;
   CU(eng->cp_level.reserve((size_t)n_in));
   CU(eng->cp_wlo.reserve((size_t)n_in));
   CU(eng->cp_whi.reserve((size_t)n_in));
   CU(eng->cp_slow.reserve((size_t)n_in));
   CU(eng->cp_cmax.reserve((size_t)n_in));
   CU(eng->cp_act.reserve((size_t)kCpMaxLevels));
-  rc = trace_join(eng, dev, h, assign, in_caller, eng->cp_parent.p, out->root, eng->cp_size.p, "tw_critical_paths", s);
+  rc = trace_join(eng, dev, h, assign, in_caller, nullptr, out->root, nullptr, "tw_critical_paths", s);
   if (rc) return rc;
   // Depth of the trees from the rounds: when round k moved no node, every node had reached its root in
   // rounds 0 .. k - 1, which climb 2^k links (none when k = 0); an in-span at depth 2m links is walked at
@@ -807,7 +813,7 @@ int tw_critical_paths(tw_engine* eng, const tw_batch* dev, const tw_batch* h, co
   if (eng->cp_force_levels) levels = eng->cp_force_levels;
   eng->cp_levels = levels;
   CpScratch sc{eng->cp_level.p, eng->cp_wlo.p, eng->cp_whi.p, eng->cp_slow.p, eng->cp_cmax.p, eng->cp_act.p};
-  CU(launch_critical_paths(*dev, f64, assign, eng->trace_claim.p, eng->cp_parent.p, slow_us, *out, sc, levels,
+  CU(launch_critical_paths(*dev, f64, assign, eng->trace_claim.p, eng->trace_parent.p, slow_us, *out, sc, levels,
                            eng->n_sm, s, eng->launches));
   return TW_OK;
 }
@@ -824,15 +830,12 @@ int tw_request_confidence(tw_engine* eng, const tw_batch* dev, const tw_batch* h
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream_;
   CU(cudaSetDevice(eng->device));
-  const int64_t n_in = h->n_in_total, n_nodes = n_in + h->n_out_total;
-  CU(eng->cp_parent.reserve((size_t)n_nodes));
-  CU(eng->cp_size.reserve((size_t)n_nodes));
+  const int64_t n_in = h->n_in_total;
   CU(eng->cf_wbits.reserve((size_t)n_in));
   CU(eng->cf_seg_conf.reserve((size_t)h->n_problems));
   CU(eng->cf_seg_req.reserve((size_t)h->n_problems));
   CU(eng->cf_flag.reserve(1));
-  rc = trace_join(eng, dev, h, assign, in_caller, eng->cp_parent.p, out->root, eng->cp_size.p,
-                  "tw_request_confidence", s);
+  rc = trace_join(eng, dev, h, assign, in_caller, nullptr, out->root, nullptr, "tw_request_confidence", s);
   if (rc) return rc;
   CfScratch sc{eng->cf_wbits.p, eng->cf_seg_conf.p, eng->cf_seg_req.p, eng->cf_flag.p};
   CU(launch_request_confidence(*dev, assign, score, code, *top, *out, sc, eng->n_sm, s, eng->launches));

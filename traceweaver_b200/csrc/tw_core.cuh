@@ -12,6 +12,7 @@
 #include <stdint.h>
 #include <string.h>
 #include <math.h>
+#include <type_traits>
 
 #include "../../include/traceweaver_b200.h"
 
@@ -745,6 +746,17 @@ TW_HD int upper_bound(const int64_t* a, int n, int64_t key) {
   while (lo < hi) {
     int mid = (lo + hi) >> 1;
     if (key < a[mid]) hi = mid; else lo = mid + 1;
+  }
+  return lo;
+}
+// last index in [0, n) with off[idx] <= key, for ascending offsets with off[0] <= key: the segment of an
+// offset table that holds element `key`.  The key is not deduced; it converts to the offsets' type.
+template <class T>
+TW_HD int last_le(const T* off, int n, std::common_type_t<T> key) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (off[mid] <= key) lo = mid; else hi = mid;
   }
   return lo;
 }

@@ -15,8 +15,6 @@ namespace tw {
 
 namespace {
 
-constexpr int kCpThreads = 256;
-
 template <class T>
 struct CpTimes {
   const T* in_s;
@@ -24,15 +22,6 @@ struct CpTimes {
   const T* out_s;
   const T* out_e;
 };
-
-__device__ __forceinline__ int cp_last_le(const int64_t* off, int n, int64_t key) {   // last idx with off[idx] <= key
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= key) lo = mid; else hi = mid;
-  }
-  return lo;
-}
 
 // In-span x on the path with window [a, b]: its self time, its chosen out-spans' self times, and the
 // windows of the callee in-spans that go on the path, whose level words become `mark` (returns their
@@ -42,7 +31,7 @@ __device__ int cp_visit(const tw_batch& bt, const CpTimes<T>& t, const int32_t* 
                         const int32_t* __restrict__ claim, const tw_critical_out& out, T* wlo, T* whi,
                         int32_t* level, int32_t x, T a, T b, int mark) {
   const int32_t n_in = (int32_t)bt.n_in_total;
-  const int p = cp_last_le(bt.prob_in_off, bt.n_problems, x);
+  const int p = last_le(bt.prob_in_off, bt.n_problems, x);
   const int64_t in0 = bt.prob_in_off[p], n = bt.prob_in_off[p + 1] - in0, i = x - in0;
   const int ep0 = bt.prob_ep_off[p], E = bt.prob_ep_off[p + 1] - ep0;
   bool has[TW_MAX_E], on[TW_MAX_E];
@@ -94,7 +83,7 @@ struct CpTail {
   int ep0;                                       // and the service's first global callee
 
   __device__ int enter(int32_t y) {
-    const int p = cp_last_le(bt.prob_in_off, bt.n_problems, y);
+    const int p = last_le(bt.prob_in_off, bt.n_problems, y);
     const int64_t in0 = bt.prob_in_off[p];
     tup = bt.prob_tuple_off[p];
     n = bt.prob_in_off[p + 1] - in0;
@@ -116,8 +105,8 @@ struct CpTail {
   __device__ int32_t up(int32_t y, int* e) const {
     const int32_t k = parent[y];                 // y's caller: out-span node n_in + its index
     const int32_t x = parent[k];
-    const int ep = cp_last_le(bt.ep_out_off, bt.n_ep_total, (int64_t)k - bt.n_in_total);
-    *e = ep - bt.prob_ep_off[cp_last_le(bt.prob_in_off, bt.n_problems, x)];
+    const int ep = last_le(bt.ep_out_off, bt.n_ep_total, (int64_t)k - bt.n_in_total);
+    *e = ep - bt.prob_ep_off[last_le(bt.prob_in_off, bt.n_problems, x)];
     return x;
   }
 };
@@ -128,7 +117,7 @@ struct CpTail {
 // (cp_tail_walk), at any depth.  Level 0 also sets culprit[] to INT_MAX for a root and -1 otherwise, flags
 // the slow requests and counts the requests.
 template <class T>
-__global__ void __launch_bounds__(kCpThreads)
+__global__ void __launch_bounds__(kTreeThreads)
 k_cp_level(tw_batch bt, CpTimes<T> t, const int32_t* __restrict__ assign, const int32_t* __restrict__ claim,
            const int32_t* __restrict__ parent, tw_critical_out out, CpScratch sc, int L, int last, double slow_us) {
   if (L > 0 && *(volatile int*)&sc.act[L - 1] == 0) return;
@@ -176,7 +165,7 @@ k_cp_level(tw_batch bt, CpTimes<T> t, const int32_t* __restrict__ assign, const 
 
 // cmax[r]: the largest self-time bits over the on-path nodes of request r (non-negative doubles order as
 // their bits)
-__global__ void __launch_bounds__(kCpThreads)
+__global__ void __launch_bounds__(kTreeThreads)
 k_cp_culprit_max(int64_t n_nodes, const uint8_t* __restrict__ on_path, const int32_t* __restrict__ root,
                  const double* __restrict__ self, unsigned long long* __restrict__ cmax) {
   for (int64_t x = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; x < n_nodes; x += (int64_t)gridDim.x * blockDim.x)
@@ -184,7 +173,7 @@ k_cp_culprit_max(int64_t n_nodes, const uint8_t* __restrict__ on_path, const int
 }
 
 // culprit[r]: the smallest on-path node of request r whose self time is cmax[r]
-__global__ void __launch_bounds__(kCpThreads)
+__global__ void __launch_bounds__(kTreeThreads)
 k_cp_culprit_min(int64_t n_nodes, const uint8_t* __restrict__ on_path, const int32_t* __restrict__ root,
                  const double* __restrict__ self, const unsigned long long* __restrict__ cmax,
                  int32_t* __restrict__ culprit) {
@@ -195,14 +184,13 @@ k_cp_culprit_min(int64_t n_nodes, const uint8_t* __restrict__ on_path, const int
   }
 }
 
-// One CTA per segment: services p < P (their in-span nodes), then callees ep (their out-span nodes).
-// Thread t adds the nodes t, t + 256, ... in order, then a butterfly per warp and the warps in order.
-__global__ void __launch_bounds__(kCpThreads)
+// One CTA per segment: services p < P (their in-span nodes), then callees ep (their out-span nodes), each
+// summed in tree_cta_sum's fixed order: column 0 all on-path nodes, column 1 those of slow requests.
+__global__ void __launch_bounds__(kTreeThreads)
 k_cp_reduce(tw_batch bt, const uint8_t* __restrict__ slow, tw_critical_out out) {
-  __shared__ double ws[2][kCpThreads / 32];
-  __shared__ int wc[2][kCpThreads / 32];
+  __shared__ double ws[2][kTreeThreads / 32];
+  __shared__ int wc[2][kTreeThreads / 32];
   const int P = bt.n_problems, n_seg = P + bt.n_ep_total;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int sg = blockIdx.x; sg < n_seg; sg += gridDim.x) {
     int64_t lo, hi;
     if (sg < P) {
@@ -212,66 +200,39 @@ k_cp_reduce(tw_batch bt, const uint8_t* __restrict__ slow, tw_critical_out out) 
       lo = bt.n_in_total + bt.ep_out_off[sg - P];
       hi = bt.n_in_total + bt.ep_out_off[sg - P + 1];
     }
-    double s0 = 0.0, s1 = 0.0;
-    int c0 = 0, c1 = 0;
-    for (int64_t x = lo + threadIdx.x; x < hi; x += blockDim.x) {
-      if (!out.on_path[x]) continue;
+    double s[2];
+    int c[2];
+    tree_cta_sum(lo, hi, [&](int64_t x, double* a, int* k) {
+      if (!out.on_path[x]) return;
       const double v = out.self_us[x];
-      s0 = dadd(s0, v);
-      ++c0;
+      a[0] = dadd(a[0], v);
+      ++k[0];
       if (slow[out.root[x]]) {
-        s1 = dadd(s1, v);
-        ++c1;
+        a[1] = dadd(a[1], v);
+        ++k[1];
       }
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) {
-      s0 = dadd(s0, __shfl_xor_sync(0xffffffffu, s0, d));
-      s1 = dadd(s1, __shfl_xor_sync(0xffffffffu, s1, d));
-      c0 += __shfl_xor_sync(0xffffffffu, c0, d);
-      c1 += __shfl_xor_sync(0xffffffffu, c1, d);
-    }
-    if (lane == 0) {
-      ws[0][warp] = s0;
-      ws[1][warp] = s1;
-      wc[0][warp] = c0;
-      wc[1][warp] = c1;
-    }
-    __syncthreads();
+    }, ws, wc, s, c);
     if (threadIdx.x == 0) {
-      for (int w = 1; w < kCpThreads / 32; ++w) {
-        s0 = dadd(s0, ws[0][w]);
-        s1 = dadd(s1, ws[1][w]);
-        c0 += wc[0][w];
-        c1 += wc[1][w];
-      }
       if (sg < P) {
-        out.server_us[2 * sg] = s0;
-        out.server_us[2 * sg + 1] = s1;
-        out.server_visits[2 * sg] = c0;
-        out.server_visits[2 * sg + 1] = c1;
+        out.server_us[2 * sg] = s[0];
+        out.server_us[2 * sg + 1] = s[1];
+        out.server_visits[2 * sg] = c[0];
+        out.server_visits[2 * sg + 1] = c[1];
       } else {
-        out.call_us[2 * (sg - P)] = s0;
-        out.call_us[2 * (sg - P) + 1] = s1;
+        out.call_us[2 * (sg - P)] = s[0];
+        out.call_us[2 * (sg - P) + 1] = s[1];
       }
     }
-    __syncthreads();
   }
-}
-
-unsigned cp_grid(int64_t n, int n_sm) {
-  const int64_t want = (n + kCpThreads - 1) / kCpThreads;
-  const int64_t cap = (int64_t)n_sm * 16;
-  return (unsigned)(want < 1 ? 1 : (want < cap ? want : cap));
 }
 
 template <class T>
 cudaError_t launch_walk(const tw_batch& b, const CpTimes<T>& t, const int32_t* assign, const int32_t* claim,
                         const int32_t* parent, double slow_us, const tw_critical_out& out, const CpScratch& sc,
                         int levels, int n_sm, cudaStream_t s, int64_t& launches) {
-  const unsigned g = cp_grid(b.n_in_total, n_sm);
+  const unsigned g = tree_grid(b.n_in_total, n_sm);
   for (int L = 0; L < levels; ++L) {
-    k_cp_level<T><<<g, kCpThreads, 0, s>>>(b, t, assign, claim, parent, out, sc, L, L == levels - 1, slow_us);
+    k_cp_level<T><<<g, kTreeThreads, 0, s>>>(b, t, assign, claim, parent, out, sc, L, L == levels - 1, slow_us);
     const cudaError_t e = after_launch(launches);
     if (e != cudaSuccess) return e;
   }
@@ -299,14 +260,14 @@ cudaError_t launch_critical_paths(const tw_batch& b, const tw_times_f64* f64, co
     e = launch_walk<int64_t>(b, CpTimes<int64_t>{b.in_start, b.in_end, b.out_start, b.out_end}, assign, claim,
                              parent, slow_us, out, sc, levels, n_sm, s, launches);
   if (e != cudaSuccess) return e;
-  const unsigned g = cp_grid(n_nodes, n_sm);
-  k_cp_culprit_max<<<g, kCpThreads, 0, s>>>(n_nodes, out.on_path, out.root, out.self_us, sc.cmax);
+  const unsigned g = tree_grid(n_nodes, n_sm);
+  k_cp_culprit_max<<<g, kTreeThreads, 0, s>>>(n_nodes, out.on_path, out.root, out.self_us, sc.cmax);
   if ((e = after_launch(launches)) != cudaSuccess) return e;
-  k_cp_culprit_min<<<g, kCpThreads, 0, s>>>(n_nodes, out.on_path, out.root, out.self_us, sc.cmax, out.culprit);
+  k_cp_culprit_min<<<g, kTreeThreads, 0, s>>>(n_nodes, out.on_path, out.root, out.self_us, sc.cmax, out.culprit);
   if ((e = after_launch(launches)) != cudaSuccess) return e;
   const int64_t n_seg = (int64_t)b.n_problems + b.n_ep_total;
   const int64_t cap = (int64_t)n_sm * 8;
-  k_cp_reduce<<<(unsigned)(n_seg < cap ? n_seg : cap), kCpThreads, 0, s>>>(b, sc.slow, out);
+  k_cp_reduce<<<(unsigned)(n_seg < cap ? n_seg : cap), kTreeThreads, 0, s>>>(b, sc.slow, out);
   return after_launch(launches);
 }
 

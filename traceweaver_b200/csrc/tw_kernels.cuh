@@ -252,6 +252,49 @@ cudaError_t launch_accuracy(const tw_batch& b, const int32_t* truth, const int32
                             unsigned long long* trace_first, unsigned long long* out4, cudaStream_t s,
                             int64_t& launches);
 
+// ---- request trees: the join (tw_traces.cu) and the analyses after it (tw_critical_path.cu,
+// tw_confidence.cu).  CTAs of kTreeThreads threads; a grid-stride grid of one thread per item, at most 16
+// CTAs per SM.
+constexpr int kTreeThreads = 256;
+inline unsigned tree_grid(int64_t n, int n_sm) {
+  const int64_t want = (n + kTreeThreads - 1) / kTreeThreads;
+  const int64_t cap = (int64_t)n_sm * 16;
+  return (unsigned)(want < 1 ? 1 : (want < cap ? want : cap));
+}
+
+// The CTA's fixed-order sums over [lo, hi) of N double / int column pairs: v(x, s, c) adds element x into
+// s[0 .. N) and c[0 .. N).  Thread t adds the elements t, t + 256, ... in order, then a butterfly per warp
+// and the warps in order; thread 0 gets the sums.  ws / wc: the kernel's shared memory.
+template <int N, class F>
+__device__ void tree_cta_sum(int64_t lo, int64_t hi, F v, double (*ws)[kTreeThreads / 32],
+                             int (*wc)[kTreeThreads / 32], double (&s)[N], int (&c)[N]) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int q = 0; q < N; ++q) {
+    s[q] = 0.0;
+    c[q] = 0;
+  }
+  for (int64_t x = lo + threadIdx.x; x < hi; x += blockDim.x) v(x, s, c);
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1)
+    for (int q = 0; q < N; ++q) {
+      s[q] = dadd(s[q], __shfl_xor_sync(0xffffffffu, s[q], d));
+      c[q] += __shfl_xor_sync(0xffffffffu, c[q], d);
+    }
+  if (lane == 0)
+    for (int q = 0; q < N; ++q) {
+      ws[q][warp] = s[q];
+      wc[q][warp] = c[q];
+    }
+  __syncthreads();
+  if (threadIdx.x == 0)
+    for (int w = 1; w < kTreeThreads / 32; ++w)
+      for (int q = 0; q < N; ++q) {
+        s[q] = dadd(s[q], ws[q][w]);
+        c[q] += wc[q][w];
+      }
+  __syncthreads();
+}
+
 // tw_traces.cu: pointer-jumping rounds for n_nodes nodes, ceil(log2 n_nodes) + 1, and the launches of
 // tw_assemble_traces.  claim: [n_out] scratch; err: 4 words (twice-claimed out-span, twice-named caller,
 // in-span with an assign index out of range, in-span whose caller is not an out-span node: the smallest

@@ -15,14 +15,10 @@ constexpr int kTimesThreads = 256;
 // Problem of element j of [in-spans | out-spans]: offsets are strictly increasing (n_in >= 2, n_out >= 1).
 __device__ __forceinline__ int elem_problem(const tw_batch& b, const int32_t* __restrict__ ep_prob, int64_t j) {
   const int64_t* off = b.prob_in_off;
-  int hi = b.n_problems;
-  if (j >= b.n_in_total) { j -= b.n_in_total; off = b.ep_out_off; hi = b.n_ep_total; }
-  int lo = 0;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= j) lo = mid; else hi = mid;
-  }
-  return off == b.prob_in_off ? lo : ep_prob[lo];
+  int n = b.n_problems;
+  if (j >= b.n_in_total) { j -= b.n_in_total; off = b.ep_out_off; n = b.n_ep_total; }
+  const int k = last_le(off, n, j);
+  return off == b.prob_in_off ? k : ep_prob[k];
 }
 
 // Bits after the binary point of x (0 for integers and zero) and floor(log2 |x|) (very negative for
@@ -118,12 +114,7 @@ k_params_scale(int mode, const int64_t* __restrict__ prob_gauss_off, int n_probl
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n_rec) return;
   if (mode == TW_PARAMS_GAUSS_BATCHED) {
-    int lo = 0, hi = n_problems;
-    while (hi - lo > 1) {
-      const int mid = (lo + hi) >> 1;
-      if (prob_gauss_off[mid] <= r) lo = mid; else hi = mid;
-    }
-    const int s = prob_shift[lo];
+    const int s = prob_shift[last_le(prob_gauss_off, n_problems, r)];
     const double* a = src + r * TW_GAUSS_REC;
     double* d = dst + r * TW_GAUSS_REC;
     d[0] = ldexp(a[0], s);

@@ -13,17 +13,6 @@ namespace tw {
 
 namespace {
 
-constexpr int kTraceThreads = 256;
-
-__device__ __forceinline__ int last_le(const int64_t* off, int n, int64_t key) {   // last idx with off[idx] <= key
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= key) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 // One thread per tuple (problem p, callee e, in-span i): assign = j >= 0 makes in-span i the parent of
 // out-span j of callee e.  parent[] of the out-spans starts at -1 and is the claim word: a second claim
 // finds it taken.  err[0]: smallest out-span node claimed twice; err[2]: smallest in-span node with an
@@ -111,12 +100,6 @@ __global__ void k_roots(int32_t n_nodes, const int32_t* __restrict__ parent, int
   }
 }
 
-unsigned grid_for(int64_t n, int n_sm) {
-  const int64_t want = (n + kTraceThreads - 1) / kTraceThreads;
-  const int64_t cap = (int64_t)n_sm * 16;
-  return (unsigned)(want < 1 ? 1 : (want < cap ? want : cap));
-}
-
 }  // namespace
 
 int trace_rounds(int64_t n_nodes) {
@@ -135,16 +118,16 @@ cudaError_t launch_assemble_traces(const tw_batch& b, int64_t n_tuple, const int
   if ((e = cudaMemsetAsync(err, 0x7f, 4 * sizeof(int32_t), s)) != cudaSuccess) return e;
   if ((e = cudaMemsetAsync(changed, 0, (size_t)rounds * sizeof(int), s)) != cudaSuccess) return e;
   if ((e = cudaMemsetAsync(size, 0, (size_t)n_nodes * sizeof(int32_t), s)) != cudaSuccess) return e;
-  k_link_out<<<grid_for(n_tuple, n_sm), kTraceThreads, 0, s>>>(b, assign, parent, err);
+  k_link_out<<<tree_grid(n_tuple, n_sm), kTreeThreads, 0, s>>>(b, assign, parent, err);
   if ((e = after_launch(launches)) != cudaSuccess) return e;
-  k_link_in<<<grid_for(n_in, n_sm), kTraceThreads, 0, s>>>(n_in, n_nodes, in_caller, parent, claim, err);
+  k_link_in<<<tree_grid(n_in, n_sm), kTreeThreads, 0, s>>>(n_in, n_nodes, in_caller, parent, claim, err);
   if ((e = after_launch(launches)) != cudaSuccess) return e;
-  const unsigned g = grid_for(n_nodes, n_sm);
+  const unsigned g = tree_grid(n_nodes, n_sm);
   for (int r = 0; r < rounds; ++r) {
-    k_jump<<<g, kTraceThreads, 0, s>>>(n_nodes, r, parent, root, changed);
+    k_jump<<<g, kTreeThreads, 0, s>>>(n_nodes, r, parent, root, changed);
     if ((e = after_launch(launches)) != cudaSuccess) return e;
   }
-  k_roots<<<g, kTraceThreads, 0, s>>>(n_nodes, parent, root, size);
+  k_roots<<<g, kTreeThreads, 0, s>>>(n_nodes, parent, root, size);
   return after_launch(launches);
 }
 

@@ -15,26 +15,13 @@ namespace tw {
 // Table of problem p: tab[tab_off[p] + e * range_p + (trace - lo_p)] = smallest list position of a span
 // of that trace in callee e's list (GetGroundTruth takes the FIRST match in list order, utils.py:28-31);
 // only traces of the problem's own in-spans (lo_p <= trace < lo_p + range_p) can match.
-__device__ __forceinline__ int last_le(const int64_t* off, int n, int64_t key) {   // last index with off[idx] <= key
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= key) lo = mid; else hi = mid;
-  }
-  return lo;
-}
 __global__ void k_truth_scatter(tw_batch b, const int32_t* __restrict__ out_trace, const int32_t* __restrict__ trace_lo,
                                 const int32_t* __restrict__ trace_n, const int64_t* __restrict__ tab_off,
                                 int32_t* __restrict__ tab) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= b.n_out_total) return;
   const int ep = last_le(b.ep_out_off, b.n_ep_total, j);
-  int lo = 0, hi = b.n_problems;               // problem of the ep
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (b.prob_ep_off[mid] <= ep) lo = mid; else hi = mid;
-  }
-  const int p = lo;
+  const int p = last_le(b.prob_ep_off, b.n_problems, ep);
   const int t = out_trace[j] - trace_lo[p];
   if (t >= 0 && t < trace_n[p])
     atomicMin(&tab[tab_off[p] + (int64_t)(ep - b.prob_ep_off[p]) * trace_n[p] + t], (int32_t)(j - b.ep_out_off[ep]));

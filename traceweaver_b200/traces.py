@@ -9,6 +9,7 @@ batch.  A node without a parent is a root: an in-span root is a reconstructed re
 detached fragment.  root[x] is -1 for a node on or under a cycle of links, size[r] counts the nodes of root
 r.  Trace ids are never read here; they enter only `exact_requests`, the comparison with the truth."""
 import ctypes as C
+from types import SimpleNamespace
 from typing import Sequence
 
 import numpy as np
@@ -48,36 +49,55 @@ def caller_links(services: Sequence, hb) -> np.ndarray:
     return out
 
 
+def upload_inputs(engine, hb, who, **arrays):
+    """The input arrays of the request-tree entry points on the engine's device, by name: assign, in_caller,
+    score, code, topk_score, topk_idx, topk_cnt (device tensors or host arrays), each flat and contiguous in
+    the dtype the kernels read.  ValueError naming the wrapper `who` and the array when its size does not fit
+    the batch `hb`."""
+    n_tuple, n_in, K = int(hb.prob_tuple_off[-1]), int(hb.prob_in_off[-1]), _abi.TW_K
+    want = dict(assign=(n_tuple, np.int32, torch.int32), in_caller=(n_in, np.int32, torch.int32),
+                score=(n_in, np.float64, torch.float64), code=(n_in, np.uint8, torch.uint8),
+                topk_score=(K * n_in, np.float64, torch.float64), topk_idx=(K * n_tuple, np.int32, torch.int32),
+                topk_cnt=(n_in, np.uint8, torch.uint8))
+    dev = engine.device
+    d = {}
+    for name, a in arrays.items():
+        size, npt, tt = want[name]
+        if isinstance(a, torch.Tensor):
+            t = a.to(device=dev, dtype=tt).contiguous().reshape(-1)
+        else:
+            t = _to_device({name: np.ascontiguousarray(np.asarray(a, npt).reshape(-1))}, dev)[name]
+        if t.numel() != size:
+            raise ValueError(f"{who}: {name} must have {size} entries for this batch, not {t.numel()}")
+        d[name] = t
+    return d
+
+
+def _batch_structs(engine, hb, spans=None):
+    """The TwBatch of `hb`'s offset tables on the device and on the host, the device one also pointing at
+    `spans` (upload_spans) when given: all the request-tree entry points read of a batch.  Also the device
+    tensors, which must outlive the call."""
+    view = SimpleNamespace(n_problems=hb.n_problems, arrays={k: hb.arrays[k] for k in _OFFSETS})
+    d = _to_device(view.arrays, engine.device)
+    host_s = batch_struct(view, lambda k: hb.arrays[k].ctypes.data)
+    if spans is not None:
+        d.update(spans)
+        view.arrays.update(spans)
+    return batch_struct(view, lambda k: d[k].data_ptr()), host_s, d
+
+
 def assemble(engine, hb, assign, in_caller):
     """tw_assemble_traces on the batch `hb` (host offsets; it need not be bound, a bound batch is not
     touched).  assign: the tw_pass_out.assign layout, in_caller: int32 [n_in]; device tensors or host
     arrays.  Returns device int32 tensors parent, root, size [n_nodes]."""
-    dev = engine.device
-    d = _to_device({k: hb.arrays[k] for k in _OFFSETS}, dev)
-    links = {}
-    for name, a in (("assign", assign), ("in_caller", in_caller)):
-        links[name] = a if isinstance(a, torch.Tensor) else _to_device({name: np.asarray(a, np.int32).reshape(-1)},
-                                                                        dev)[name]
-    n_tuple, n_in = int(hb.prob_tuple_off[-1]), int(hb.prob_in_off[-1])
-    if links["assign"].numel() != n_tuple or links["in_caller"].numel() != n_in:
-        raise ValueError(f"assemble: assign must have {n_tuple} entries and in_caller {n_in}")
-    view = _OffsetView(hb)
-    dev_s = batch_struct(view, lambda k: d[k].data_ptr())
-    host_s = batch_struct(view, lambda k: hb.arrays[k].ctypes.data)
+    links = upload_inputs(engine, hb, "assemble", assign=assign, in_caller=in_caller)
+    dev_s, host_s, _keep = _batch_structs(engine, hb)
     n = node_count(hb)
-    out = {k: torch.empty(n, dtype=torch.int32, device=dev) for k in ("parent", "root", "size")}
+    out = {k: torch.empty(n, dtype=torch.int32, device=engine.device) for k in ("parent", "root", "size")}
     _lib.check(engine.lib.tw_assemble_traces(engine.h, C.byref(dev_s), C.byref(host_s), _p(links["assign"]),
                                              _p(links["in_caller"]), _p(out["parent"]), _p(out["root"]),
                                              _p(out["size"]), engine.stream), "tw_assemble_traces")
     return out
-
-
-class _OffsetView:
-    """The offset tables of a batch, without its span arrays or term tables: all tw_assemble_traces reads."""
-
-    def __init__(self, hb):
-        self.arrays = {k: hb.arrays[k] for k in _OFFSETS}
-        self.n_problems = hb.n_problems
 
 
 def exact_requests(root_pred: torch.Tensor, root_true: torch.Tensor, n_in: int) -> torch.Tensor:
@@ -98,6 +118,17 @@ def exact_requests(root_pred: torch.Tensor, root_true: torch.Tensor, n_in: int) 
 # Host restatement: the same arrays by walking each node up to its root (the reference the tests compare
 # tw_assemble_traces with; no GPU needed).
 # ---------------------------------------------------------------------------------------------
+def _tuples(hb):
+    """Every tuple g = tuple_off[p] + e * n_p + i of the batch (service p, callee position e, in-span i) as
+    its global callee ep, its callee position e and its in-span node: three int64 arrays [n_tuple]."""
+    off = np.asarray(hb.prob_tuple_off, np.int64)
+    p = np.repeat(np.arange(hb.n_problems), np.diff(off))
+    n_p = np.diff(np.asarray(hb.prob_in_off, np.int64))[p]
+    local = np.arange(off[-1]) - off[p]
+    pos = local // n_p
+    return np.asarray(hb.prob_ep_off, np.int64)[p] + pos, pos, np.asarray(hb.prob_in_off, np.int64)[p] + local % n_p
+
+
 def _smallest_repeat(x):
     v, c = np.unique(x, return_counts=True)
     return int(v[c > 1][0]) if (c > 1).any() else None
@@ -116,13 +147,7 @@ def parents_host(hb, assign, in_caller) -> np.ndarray:
     if twice is not None:
         raise ValueError(f"out-span node {twice} is the caller of two in-spans")
     parent[:n_in] = c
-    # tuple g = (service p, callee e, in-span i), g = tuple_off[p] + e * n_p + i
-    off = np.asarray(hb.prob_tuple_off, np.int64)
-    p = np.repeat(np.arange(hb.n_problems), np.diff(off))
-    n_p = np.diff(np.asarray(hb.prob_in_off, np.int64))[p]
-    local = np.arange(off[-1]) - off[p]
-    ep = np.asarray(hb.prob_ep_off, np.int64)[p] + local // n_p
-    node_in = np.asarray(hb.prob_in_off, np.int64)[p] + local % n_p
+    ep, _, node_in = _tuples(hb)
     out_off = np.asarray(hb.ep_out_off, np.int64)
     has = assign >= 0
     outside = np.flatnonzero(has & (assign >= out_off[ep + 1] - out_off[ep]))
@@ -197,14 +222,6 @@ def upload_spans(engine, hb):
     return _to_device({k: hb.arrays[k] for k in SPAN_ARRAYS}, engine.device)
 
 
-class _SpanView(_OffsetView):
-    """The offset tables and span arrays of a batch: all tw_critical_paths reads."""
-
-    def __init__(self, hb, spans):
-        super().__init__(hb)
-        self.arrays.update(spans)
-
-
 def critical_paths(engine, hb, assign, in_caller, slow_us, spans=None):
     """tw_critical_paths on the batch `hb` (host offsets; it need not be bound, a bound batch is not
     touched).  assign, in_caller as for assemble; slow_us: requests with latency >= slow_us form the second
@@ -213,20 +230,11 @@ def critical_paths(engine, hb, assign, in_caller, slow_us, spans=None):
     [P, 2], server_visits int32 [P, 2], call_us float64 [n_ep, 2], requests int32 [2].  Trees of any depth
     are walked, with the same results whatever the number of level launches."""
     dev = engine.device
-    d = _to_device({k: hb.arrays[k] for k in _OFFSETS}, dev)
-    d.update(spans if spans is not None else upload_spans(engine, hb))
-    links = {}
-    for name, a in (("assign", assign), ("in_caller", in_caller)):
-        links[name] = a if isinstance(a, torch.Tensor) else _to_device({name: np.asarray(a, np.int32).reshape(-1)},
-                                                                        dev)[name]
-    n_tuple, n_in = int(hb.prob_tuple_off[-1]), int(hb.prob_in_off[-1])
-    if links["assign"].numel() != n_tuple or links["in_caller"].numel() != n_in:
-        raise ValueError(f"critical_paths: assign must have {n_tuple} entries and in_caller {n_in}")
-    view = _SpanView(hb, {k: d[k] for k in SPAN_ARRAYS})
-    dev_s = batch_struct(view, lambda k: d[k].data_ptr())
-    host_s = batch_struct(_OffsetView(hb), lambda k: hb.arrays[k].ctypes.data)
-    f64 = _abi.fill(_abi.TwTimesF64, d) if d["in_start"].dtype == torch.float64 else None
-    n, P, n_ep = node_count(hb), hb.n_problems, int(hb.prob_ep_off[-1])
+    links = upload_inputs(engine, hb, "critical_paths", assign=assign, in_caller=in_caller)
+    spans = spans if spans is not None else upload_spans(engine, hb)
+    dev_s, host_s, _keep = _batch_structs(engine, hb, spans)
+    f64 = _abi.fill(_abi.TwTimesF64, spans) if spans["in_start"].dtype == torch.float64 else None
+    n, n_in, P, n_ep = node_count(hb), int(hb.prob_in_off[-1]), hb.n_problems, int(hb.prob_ep_off[-1])
     out = dict(root=torch.empty(n, dtype=torch.int32, device=dev), on_path=torch.empty(n, dtype=torch.uint8, device=dev),
                self_us=torch.empty(n, dtype=torch.float64, device=dev),
                culprit=torch.empty(n_in, dtype=torch.int32, device=dev),
@@ -272,13 +280,7 @@ def critical_paths_host(hb, assign, in_caller, slow_us):
     out_s, out_e = hb.out_start.tolist(), hb.out_end.tolist()
     # the child out-span of every in-span per callee position (-1: none), and every out-span's child in-span
     assign = np.asarray(assign, np.int64).reshape(-1)
-    off = np.asarray(hb.prob_tuple_off, np.int64)
-    p = np.repeat(np.arange(P), np.diff(off))
-    n_p = np.diff(np.asarray(hb.prob_in_off, np.int64))[p]
-    local = np.arange(off[-1]) - off[p]
-    pos = local // n_p
-    ep = np.asarray(hb.prob_ep_off, np.int64)[p] + pos
-    node_in = np.asarray(hb.prob_in_off, np.int64)[p] + local % n_p
+    ep, pos, node_in = _tuples(hb)
     kids = np.full((n_in, 8), -1, np.int64)
     has = assign >= 0
     kids[node_in[has], pos[has]] = np.asarray(hb.ep_out_off, np.int64)[ep[has]] + assign[has]
@@ -457,28 +459,11 @@ def request_confidence(engine, hb, assign, in_caller, score, code, topk):
     int32, log_conf int64 (units of 2^-32 nats), conf float64, weakest int32, weakest_p float64 [n_in];
     est_accuracy float64 [P]; requests int32 [1]; expected_exact float64 [1].  Definition above."""
     dev = engine.device
-    d = _to_device({k: hb.arrays[k] for k in _OFFSETS}, dev)
-    n_tuple, n_in = int(hb.prob_tuple_off[-1]), int(hb.prob_in_off[-1])
-    want = dict(assign=(n_tuple, np.int32, torch.int32), in_caller=(n_in, np.int32, torch.int32),
-                score=(n_in, np.float64, torch.float64), code=(n_in, np.uint8, torch.uint8),
-                topk_score=(_abi.TW_K * n_in, np.float64, torch.float64),
-                topk_idx=(_abi.TW_K * n_tuple, np.int32, torch.int32), topk_cnt=(n_in, np.uint8, torch.uint8))
-    given = dict(assign=assign, in_caller=in_caller, score=score, code=code, topk_score=topk["topk_score"],
-                 topk_idx=topk["topk_idx"], topk_cnt=topk["topk_cnt"])
-    links = {}
-    for name, a in given.items():
-        size, npt, tt = want[name]
-        if isinstance(a, torch.Tensor):
-            t = a.to(device=dev, dtype=tt).contiguous().reshape(-1)
-        else:
-            t = _to_device({name: np.ascontiguousarray(np.asarray(a, npt).reshape(-1))}, dev)[name]
-        if t.numel() != size:
-            raise ValueError(f"request_confidence: {name} must have {size} entries for this batch, not {t.numel()}")
-        links[name] = t
-    view = _OffsetView(hb)
-    dev_s = batch_struct(view, lambda k: d[k].data_ptr())
-    host_s = batch_struct(view, lambda k: hb.arrays[k].ctypes.data)
-    n, P = node_count(hb), hb.n_problems
+    links = upload_inputs(engine, hb, "request_confidence", assign=assign, in_caller=in_caller, score=score,
+                          code=code, topk_score=topk["topk_score"], topk_idx=topk["topk_idx"],
+                          topk_cnt=topk["topk_cnt"])
+    dev_s, host_s, _keep = _batch_structs(engine, hb)
+    n, n_in, P = node_count(hb), int(hb.prob_in_off[-1]), hb.n_problems
     out = dict(root=torch.empty(n, dtype=torch.int32, device=dev))
     for k, dt in (("p", torch.float64), ("ell", torch.float64), ("decisions", torch.int32), ("zero", torch.int32),
                   ("log_conf", torch.int64), ("conf", torch.float64), ("weakest", torch.int32),
