@@ -27,6 +27,11 @@ int two_windows_from_cuts(int n, const uint8_t* cut, uint8_t* win_end);
 int two_gmm_refit(int32_t n_terms, const int64_t* term_sample_off, const double* delays,
                   const int32_t* counts, uint32_t seed_select, double* mix_out,
                   int32_t* n_selected_out);
+/* the refit with every term's 'diag' BIC per component count and every fit's decisions (tw_oracle_gmm.c) */
+int two_gmm_refit_record(int32_t n_terms, const int64_t* term_sample_off, const double* delays,
+                         const int32_t* counts, uint32_t seed_select, const uint32_t* rng_skip,
+                         double* mix_out, int32_t* n_selected_out, int32_t* max_n_out, double* bic_out,
+                         int32_t* rec_out);
 /* all problems, both passes, `threads` worker threads (cpu_baseline / --impl reference) */
 int two_find_assignments(const tw_batch* b, uint32_t seed_select, int threads,
                          const tw_pass_out* final, const tw_score_out* topk_final,

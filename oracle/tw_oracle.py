@@ -14,6 +14,7 @@ from traceweaver_b200.batch import HostBatch, batch_struct
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
+_LIB_LD = None
 
 
 def build(force=False):
@@ -29,7 +30,8 @@ def build(force=False):
 def _declare(lib):
     """The return types of the oracle's entry points (every build of it: this one and tests/oracle_f64.py)."""
     for name in ("two_params_pass0", "two_score_problem", "two_stitch_problem", "two_assess_problem",
-                 "two_delays", "two_windows_from_cuts", "two_gmm_refit_ex", "two_find_assignments"):
+                 "two_delays", "two_windows_from_cuts", "two_gmm_refit_ex", "two_gmm_refit_record",
+                 "two_find_assignments"):
         getattr(lib, name).restype = C.c_int
     return lib
 
@@ -148,10 +150,30 @@ def windows_from_cuts(cut):
     return list(zip(starts.tolist(), ends.tolist()))
 
 
-def gmm_refit(term_sample_off, delays, counts, seed_select=10, rng_skip=None):
-    """two_gmm_refit_ex: per-term BIC-selected 1-D GMM (restated sklearn, oracle/tw_oracle_gmm.c).
-    Returns (mix[n_terms, TW_MIX_REC], n_selected, max_n)."""
-    L = lib()
+def _gmm_twin():
+    """libtw_oracle_gmm_ld.so: the refit alone with long double accumulators (built on first use)."""
+    global _LIB_LD
+    if _LIB_LD is None:
+        so = os.path.join(HERE, "libtw_oracle_gmm_ld.so")
+        src = [os.path.join(HERE, f) for f in ("tw_oracle_gmm.c", "tw_oracle.h")]
+        if not os.path.exists(so) or any(os.path.getmtime(f) > os.path.getmtime(so) for f in src):
+            subprocess.check_call(["make", "-s", "-C", HERE, "-B", "libtw_oracle_gmm_ld.so"])
+        _LIB_LD = C.CDLL(so)
+        _LIB_LD.two_gmm_refit_record.restype = C.c_int
+    return _LIB_LD
+
+
+GMM_REC_FIELDS = ("status", "lloyd_iter", "lloyd_strict", "relocations", "em_iter", "em_converged", "replay",
+                  "lloyd_ties")
+
+
+def gmm_refit(term_sample_off, delays, counts, seed_select=10, rng_skip=None, want_record=False, twin=False):
+    """two_gmm_refit_record: per-term BIC-selected 1-D GMM (restated sklearn, oracle/tw_oracle_gmm.c).
+    Returns (mix[n_terms, TW_MIX_REC], n_selected, max_n); with want_record also bic[n_terms, 5], the 'diag'
+    BIC of each component count (+inf where that fit is not tried or raises), and rec[n_terms, 6, 8], the
+    decisions of each fit (row k - 1: the 'diag' fit with k components, row 5: the final 'full' fit; columns
+    GMM_REC_FIELDS).  twin: the same fit with long double accumulators."""
+    L = _gmm_twin() if twin else lib()
     nt = len(counts)
     off = np.ascontiguousarray(term_sample_off, np.int64)
     delays = np.ascontiguousarray(delays, np.float64)
@@ -159,10 +181,12 @@ def gmm_refit(term_sample_off, delays, counts, seed_select=10, rng_skip=None):
     mix = np.zeros((nt, _abi.TW_MIX_REC), np.float64)
     nsel = np.zeros(nt, np.int32)
     maxn = np.zeros(nt, np.int32)
+    bic = np.zeros((nt, _abi.TW_GMM_MAX_COMP), np.float64) if want_record else None
+    rec = np.zeros((nt, _abi.TW_GMM_MAX_COMP + 1, len(GMM_REC_FIELDS)), np.int32) if want_record else None
     skip = None if rng_skip is None else np.ascontiguousarray(rng_skip, np.uint32)
-    _check(L.two_gmm_refit_ex(C.c_int32(nt), _ptr(off), _ptr(delays), _ptr(counts), C.c_uint32(seed_select),
-                              _ptr(skip), _ptr(mix), _ptr(nsel), _ptr(maxn)), "gmm_refit")
-    return mix, nsel, maxn
+    _check(L.two_gmm_refit_record(C.c_int32(nt), _ptr(off), _ptr(delays), _ptr(counts), C.c_uint32(seed_select),
+                                  _ptr(skip), _ptr(mix), _ptr(nsel), _ptr(maxn), _ptr(bic), _ptr(rec)), "gmm_refit")
+    return (mix, nsel, maxn, bic, rec) if want_record else (mix, nsel, maxn)
 
 
 def find_assignments(hb: HostBatch, seed_select=10, threads=1, want_topk=True):

@@ -40,6 +40,19 @@
 #define KM_TOL 1e-4
 #define DBL_EPS 2.220446049250313e-16
 
+/* The accumulators of every sum.  The default build keeps them double; the twin build
+ * (libtw_oracle_gmm_ld.so, -DTW_GMM_ACC="long double") widens them, so that a term whose discrete
+ * decisions or parameters move between the two builds is known to depend on summation order. */
+#ifndef TW_GMM_ACC
+#define TW_GMM_ACC double
+#endif
+typedef TW_GMM_ACC acc_t;
+
+/* what one fit decided (two_gmm_refit_record): a row of TW_GMM_REC_FIELDS int32 */
+enum { R_STATUS, R_LLOYD_ITER, R_LLOYD_STRICT, R_RELOC, R_EM_ITER, R_EM_CONVERGED, R_REPLAY, R_LLOYD_TIES,
+       TW_GMM_REC_FIELDS };
+typedef int32_t fitrec_t[TW_GMM_REC_FIELDS];
+
 /* ---- numpy legacy RandomState ----------------------------------------------------------- */
 typedef struct { uint32_t mt[624]; int idx; } mt_t;
 
@@ -66,19 +79,20 @@ static double mt_random_sample(mt_t* r) {
 }
 
 /* np.sum / np.mean over a contiguous float64 vector: pairwise summation, blocks of 128, 8 lanes */
-static double pw_sum(const double* a, int n) {
-  if (n < 8) { double r = 0.0; for (int i = 0; i < n; ++i) r += a[i]; return r; }
+static acc_t pw_acc(const double* a, int n) {
+  if (n < 8) { acc_t r = 0.0; for (int i = 0; i < n; ++i) r += a[i]; return r; }
   if (n <= 128) {
-    double r[8]; for (int j = 0; j < 8; ++j) r[j] = a[j];
+    acc_t r[8]; for (int j = 0; j < 8; ++j) r[j] = a[j];
     int i = 8;
     for (; i < n - (n % 8); i += 8) for (int j = 0; j < 8; ++j) r[j] += a[i + j];
-    double res = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
+    acc_t res = ((r[0] + r[1]) + (r[2] + r[3])) + ((r[4] + r[5]) + (r[6] + r[7]));
     for (; i < n; ++i) res += a[i];
     return res;
   }
   int n2 = n / 2; n2 -= n2 % 8;
-  return pw_sum(a, n2) + pw_sum(a + n2, n - n2);
+  return pw_acc(a, n2) + pw_acc(a + n2, n - n2);
 }
+static double pw_sum(const double* a, int n) { return (double)pw_acc(a, n); }
 
 typedef struct {
   int k;
@@ -87,13 +101,30 @@ typedef struct {
 } gmm_t;
 
 /* ---- k-means (labels only matter downstream) -------------------------------------------- */
+/* nearest centre of x (first minimum); *tie += 1 when the runner-up's c^2 - 2 x c is within 1e-12 of the
+ * terms' size: such a label follows the last bits of the centres, i.e. the summation order behind them */
+static int nearest_centre(const double* centers, const double* cn, int k, double x, int32_t* tie) {
+  int lab = 0; double best = cn[0] + (-2.0 * (x * centers[0])), second = INFINITY, scale = fabs(cn[0]);
+  for (int j = 1; j < k; ++j) {
+    double d = cn[j] + (-2.0 * (x * centers[j]));
+    if (fabs(cn[j]) > scale) scale = fabs(cn[j]);
+    if (d < best) { second = best; best = d; lab = j; }
+    else if (d < second) second = d;
+  }
+  double sx = 2.0 * fabs(x) * sqrt(scale);
+  if (sx > scale) scale = sx;
+  if (k > 1 && second - best <= 1e-12 * scale) ++*tie;
+  return lab;
+}
+
 static double sq_dist(double c, double c2, double x, double x2) { /* _euclidean_distances */
   double d = -2.0 * (c * x);
   d += c2; d += x2;
   return d > 0.0 ? d : 0.0;
 }
 
-static void kmeans_labels(const double* x_in, int n, int k, mt_t* rng, int* labels, double* work /* 4n */) {
+static void kmeans_labels(const double* x_in, int n, int k, mt_t* rng, int* labels, double* work /* 4n */,
+                          int32_t* fr) {
   double* x = work; double* x2 = work + n; double* closest = work + 2 * n; double* tmp = work + 3 * n;
   double mean = pw_sum(x_in, n) / (double)n;
   for (int i = 0; i < n; ++i) { x[i] = x_in[i] - mean; x2[i] = x[i] * x[i]; }
@@ -105,10 +136,15 @@ static void kmeans_labels(const double* x_in, int n, int k, mt_t* rng, int* labe
   double tol = var * KM_TOL;
 
   /* k-means++ seeding (_kmeans_plusplus) */
-  double centers[TW_GMM_MAX_COMP], centers_new[TW_GMM_MAX_COMP], wsum[TW_GMM_MAX_COMP];
+  double centers[TW_GMM_MAX_COMP];
+  acc_t centers_new[TW_GMM_MAX_COMP], wsum[TW_GMM_MAX_COMP];
   {
     /* random_state.choice(n, p = 1/n): cdf = cumsum(p); cdf /= cdf[-1]; searchsorted(u, 'right') */
     double u = mt_random_sample(rng);
+    /* the device's first_centre (tw_core.cuh) replays NumPy's sum only within this band of an integer */
+    { double un = u * (double)n, bound = 1e-6, b2 = (double)n * ((double)n + 5.0) * 0x1p-52;
+      if (b2 > bound) bound = b2;
+      fr[R_REPLAY] = fabs(un - rint(un)) < bound; }
     double p = 1.0 / (double)n, last = 0.0;
     { double c = 0.0; for (int i = 0; i < n; ++i) c += p; last = c; }
     int id = n - 1; double c = 0.0;
@@ -116,25 +152,27 @@ static void kmeans_labels(const double* x_in, int n, int k, mt_t* rng, int* labe
     centers[0] = x[id];
     double c2 = centers[0] * centers[0];
     for (int i = 0; i < n; ++i) closest[i] = sq_dist(centers[0], c2, x[i], x2[i]);
-    double pot = 0.0; for (int i = 0; i < n; ++i) pot += closest[i];
+    acc_t pot_a = 0.0; for (int i = 0; i < n; ++i) pot_a += closest[i];
+    double pot = (double)pot_a;
     int trials = 2 + (int)log((double)k);
     for (int cidx = 1; cidx < k; ++cidx) {
       double rv[8]; int cand[8];
       for (int t = 0; t < trials; ++t) rv[t] = mt_random_sample(rng) * pot;
       /* np.searchsorted(np.cumsum(closest), rand_vals) (side='left'), clipped */
       for (int t = 0; t < trials; ++t) {
-        double cs = 0.0; int found = n - 1;
+        acc_t cs = 0.0; int found = n - 1;
         for (int i = 0; i < n; ++i) { cs += closest[i]; if (cs >= rv[t]) { found = i; break; } }
         cand[t] = found;
       }
       int best_t = 0; double best_pot = INFINITY;
       for (int t = 0; t < trials; ++t) {
-        double cc = x[cand[t]], cc2 = cc * cc, pt = 0.0;
+        double cc = x[cand[t]], cc2 = cc * cc;
+        acc_t pt = 0.0;
         for (int i = 0; i < n; ++i) {
           double d = sq_dist(cc, cc2, x[i], x2[i]);
           pt += d < closest[i] ? d : closest[i];
         }
-        if (pt < best_pot) { best_pot = pt; best_t = t; }
+        if ((double)pt < best_pot) { best_pot = (double)pt; best_t = t; }
       }
       double cc = x[cand[best_t]], cc2 = cc * cc;
       for (int i = 0; i < n; ++i) {
@@ -153,11 +191,7 @@ static void kmeans_labels(const double* x_in, int n, int k, mt_t* rng, int* labe
     double cn[TW_GMM_MAX_COMP];
     for (int j = 0; j < k; ++j) { cn[j] = centers[j] * centers[j]; centers_new[j] = 0.0; wsum[j] = 0.0; }
     for (int i = 0; i < n; ++i) {
-      int lab = 0; double best = cn[0] + (-2.0 * (x[i] * centers[0]));
-      for (int j = 1; j < k; ++j) {
-        double d = cn[j] + (-2.0 * (x[i] * centers[j]));
-        if (d < best) { best = d; lab = j; }
-      }
+      int lab = nearest_centre(centers, cn, k, x[i], &fr[R_LLOYD_TIES]);
       labels[i] = lab; centers_new[lab] += x[i]; wsum[lab] += 1.0;
     }
     /* _relocate_empty_clusters_dense: move the farthest points into empty clusters */
@@ -166,34 +200,30 @@ static void kmeans_labels(const double* x_in, int n, int k, mt_t* rng, int* labe
       int far = 0; double fd = -1.0;
       for (int i = 0; i < n; ++i) { double d = (x[i] - centers[labels[i]]) * (x[i] - centers[labels[i]]); if (d > fd) { fd = d; far = i; } }
       int ol = labels[far];
+      ++fr[R_RELOC];
       centers_new[ol] -= x[far]; wsum[ol] -= 1.0;
       centers_new[j] = x[far]; wsum[j] = 1.0;
       x2[far] = x2[far]; /* labels are NOT updated by sklearn here */
     }
-    double shift_tot = 0.0;
+    acc_t shift_tot = 0.0;
     for (int j = 0; j < k; ++j) {
-      if (wsum[j] > 0.0) centers_new[j] = centers_new[j] * (1.0 / wsum[j]);
-      double d = centers_new[j] - centers[j]; d = fabs(d);
+      double cn_j = (double)centers_new[j];
+      if (wsum[j] > 0.0) cn_j = (double)(centers_new[j] * (1.0 / wsum[j]));
+      double d = cn_j - centers[j]; d = fabs(d);
       shift_tot += d * d;
-      centers[j] = centers_new[j];
+      centers[j] = cn_j;
     }
+    fr[R_LLOYD_ITER] = it + 1;
     int same = 1;
     for (int i = 0; i < n; ++i) if (labels[i] != labels_old[i]) { same = 0; break; }
-    if (same) { strict = 1; break; }
+    if (same) { strict = 1; fr[R_LLOYD_STRICT] = 1; break; }
     if (shift_tot <= tol) break;
     memcpy(labels_old, labels, sizeof(int) * (size_t)n);
   }
   if (!strict) {
     double cn[TW_GMM_MAX_COMP];
     for (int j = 0; j < k; ++j) cn[j] = centers[j] * centers[j];
-    for (int i = 0; i < n; ++i) {
-      int lab = 0; double best = cn[0] + (-2.0 * (x[i] * centers[0]));
-      for (int j = 1; j < k; ++j) {
-        double d = cn[j] + (-2.0 * (x[i] * centers[j]));
-        if (d < best) { best = d; lab = j; }
-      }
-      labels[i] = lab;
-    }
+    for (int i = 0; i < n; ++i) labels[i] = nearest_centre(centers, cn, k, x[i], &fr[R_LLOYD_TIES]);
   }
 }
 
@@ -212,44 +242,47 @@ static double comp_logprob(const gmm_t* g, int c, double x, int full) {
 }
 static double lse(const double* a, int k) { /* scipy.special.logsumexp */
   double amax = -INFINITY; for (int c = 0; c < k; ++c) if (a[c] > amax) amax = a[c];
-  double s = 0.0, m = 0.0;
+  acc_t s = 0.0; double m = 0.0;
   for (int c = 0; c < k; ++c) { if (a[c] == amax) m += 1.0; else s += exp(a[c] - amax); }
   if (s != 0.0) s /= m;
-  return log1p(s) + log(m) + amax;
+  return log1p((double)s) + log(m) + amax;
 }
 /* M-step / initialisation from responsibilities: returns -1 where sklearn raises ValueError */
 static int m_step(gmm_t* g, const double* x, int n, const double* resp, int full, int init) {
   int k = g->k;
   double nk[TW_GMM_MAX_COMP];
   for (int c = 0; c < k; ++c) {
-    double s = 0.0; for (int i = 0; i < n; ++i) s += resp[(size_t)i * k + c];
-    nk[c] = s + 10.0 * DBL_EPS;
-    double sx = 0.0; for (int i = 0; i < n; ++i) sx += resp[(size_t)i * k + c] * x[i];
-    g->mu[c] = sx / nk[c];
+    acc_t s = 0.0; for (int i = 0; i < n; ++i) s += resp[(size_t)i * k + c];
+    nk[c] = (double)s + 10.0 * DBL_EPS;
+    acc_t sx = 0.0; for (int i = 0; i < n; ++i) sx += resp[(size_t)i * k + c] * x[i];
+    g->mu[c] = (double)sx / nk[c];
     if (full) {
-      double sv = 0.0;
+      acc_t sv = 0.0;
       for (int i = 0; i < n; ++i) { double d = x[i] - g->mu[c]; sv += (resp[(size_t)i * k + c] * d) * d; }
-      g->cov[c] = sv / nk[c] + REG_COVAR;
+      g->cov[c] = (double)sv / nk[c] + REG_COVAR;
     } else {
-      double sx2 = 0.0; for (int i = 0; i < n; ++i) sx2 += resp[(size_t)i * k + c] * (x[i] * x[i]);
-      g->cov[c] = sx2 / nk[c] - g->mu[c] * g->mu[c] + REG_COVAR;
+      acc_t sx2 = 0.0; for (int i = 0; i < n; ++i) sx2 += resp[(size_t)i * k + c] * (x[i] * x[i]);
+      g->cov[c] = (double)(sx2 / nk[c] - (acc_t)g->mu[c] * g->mu[c]) + REG_COVAR;
     }
     if (!(g->cov[c] > 0.0)) return -1;
     g->pc[c] = 1.0 / sqrt(g->cov[c]);
   }
   if (init) { for (int c = 0; c < k; ++c) g->w[c] = nk[c] / (double)n; }
-  else { double s = 0.0; for (int c = 0; c < k; ++c) s += nk[c]; for (int c = 0; c < k; ++c) g->w[c] = nk[c] / s; }
+  else { acc_t s = 0.0; for (int c = 0; c < k; ++c) s += nk[c]; for (int c = 0; c < k; ++c) g->w[c] = nk[c] / (double)s; }
   return 0;
 }
 
 static int gmm_fit(const double* x, int n, int k, int full, mt_t* rng, gmm_t* g, double* work /* 4n + n*k */,
-                   int* labels) {
+                   int* labels, int32_t* fr) {
+  memset(fr, 0, sizeof(fitrec_t));
   if (n < 2 || n < k) { /* sklearn: ensure_min_samples=2 / n_samples >= n_components */
     /* the k-means draw is never reached */
+    fr[R_STATUS] = -1;
     return -1;
   }
+  fr[R_STATUS] = -2;    /* ValueError from a non-positive covariance, unless the fit completes */
   g->k = k;
-  kmeans_labels(x, n, k, rng, labels, work);
+  kmeans_labels(x, n, k, rng, labels, work, fr);
   double* resp = work + 4 * (size_t)n;
   for (int i = 0; i < n; ++i) for (int c = 0; c < k; ++c) resp[(size_t)i * k + c] = labels[i] == c ? 1.0 : 0.0;
   if (m_step(g, x, n, resp, full, 1)) return -1;
@@ -266,10 +299,13 @@ static int gmm_fit(const double* x, int n, int k, int full, mt_t* rng, gmm_t* g,
       for (int c = 0; c < k; ++c) resp[(size_t)i * k + c] = exp(a[c] - l);
     }
     lower = pw_sum(lpn, n) / (double)n;
+    fr[R_EM_ITER] = it;
     if (m_step(g, x, n, resp, full, 0)) return -1;
     g->n_iter = it;
     if (fabs(lower - prev) < EM_TOL) { g->converged = 1; break; }
   }
+  fr[R_EM_CONVERGED] = g->converged;
+  fr[R_STATUS] = 1;
   return 0;
 }
 
@@ -294,13 +330,18 @@ int two_gmm_draws_for(int max_n) {
   return tot;
 }
 
-/* One term: returns n_selected (0 = degenerate Gaussian record) */
+/* One term: returns n_selected (0 = degenerate Gaussian record).  bic (may be NULL) gets the 'diag' BIC
+ * of every K = 1..5, +inf where the fit is not tried or raises. */
 static int refit_term(const double* x, int n, uint32_t seed_select, uint32_t rng_skip, double* rec,
-                      int* max_n_out) {
+                      int* max_n_out, double* bic_out, int32_t* rec_out) {
+  fitrec_t frs[TW_GMM_MAX_COMP + 1];
+  memset(frs, 0, sizeof frs);
+  if (bic_out) for (int k = 0; k < TW_GMM_MAX_COMP; ++k) bic_out[k] = INFINITY;
   memset(rec, 0, sizeof(double) * TW_MIX_REC);
   if (n == 0) { /* services_times = (0, 0) -> std clamp 0.001 (V3:765-766, V1:130-131) */
     rec[0] = 0.0; rec[1] = 0.0; rec[2] = 0.001; rec[3] = log(0.001);
     *max_n_out = 0;
+    if (rec_out) memcpy(rec_out, frs, sizeof frs);
     return 0;
   }
   double* work = (double*)malloc(sizeof(double) * ((size_t)n * (5 + TW_GMM_MAX_COMP)));
@@ -316,17 +357,18 @@ static int refit_term(const double* x, int n, uint32_t seed_select, uint32_t rng
   int best_k = 0; double best_bic = INFINITY;
   for (int k = 1; k <= max_n; ++k) {
     gmm_t g;
-    if (gmm_fit(x, n, k, 0, &rng, &g, work, labels)) continue;
+    if (gmm_fit(x, n, k, 0, &rng, &g, work, labels, frs[k - 1])) continue;
     double sc = gmm_score(&g, x, n, 0, work);
     double bic = -2.0 * sc * (double)n + (double)(3 * k - 1) * log((double)n);
     if (getenv("TWO_GMM_DEBUG")) fprintf(stderr, "two_gmm: n=%d k=%d bic=%.6f\n", n, k, bic);
+    if (bic_out) bic_out[k - 1] = bic;
     if (bic < best_bic) { best_bic = bic; best_k = k; }
   }
   int ret = 0;
   if (best_k > 0) {
     mt_t r100; mt_seed(&r100, 100u);
     gmm_t g;
-    if (gmm_fit(x, n, best_k, 1, &r100, &g, work, labels) == 0) {
+    if (gmm_fit(x, n, best_k, 1, &r100, &g, work, labels, frs[TW_GMM_MAX_COMP]) == 0) {
       rec[0] = (double)best_k;
       for (int c = 0; c < best_k; ++c) {
         rec[1 + c] = g.pc[c]; rec[6 + c] = g.mu[c] * g.pc[c];
@@ -336,6 +378,7 @@ static int refit_term(const double* x, int n, uint32_t seed_select, uint32_t rng
     }
   }
   if (ret == 0) { rec[0] = 0.0; rec[1] = 0.0; rec[2] = 0.001; rec[3] = log(0.001); }
+  if (rec_out) memcpy(rec_out, frs, sizeof frs);
   free(work); free(labels);
   return ret;
 }
@@ -349,10 +392,25 @@ static int refit_term(const double* x, int n, uint32_t seed_select, uint32_t rng
 int two_gmm_refit_ex(int32_t n_terms, const int64_t* term_sample_off, const double* delays,
                      const int32_t* counts, uint32_t seed_select, const uint32_t* rng_skip,
                      double* mix_out, int32_t* n_selected_out, int32_t* max_n_out) {
+  return two_gmm_refit_record(n_terms, term_sample_off, delays, counts, seed_select, rng_skip, mix_out,
+                              n_selected_out, max_n_out, NULL, NULL);
+}
+
+/* two_gmm_refit_ex and the decisions of every fit.  bic_out[t * 5 + k - 1]: the 'diag' BIC of term t with
+ * k components (+inf where that fit is not tried or raises).  rec_out[(t * 6 + f) * 7 + field], f = k - 1
+ * for the 'diag' fits and f = 5 for the final 'full' fit; fields: status (0 not tried, -1 too few samples,
+ * -2 ValueError, 1 fitted), Lloyd iterations, Lloyd stopped on unchanged labels (1) or on the centre
+ * shift (0), empty-cluster relocations, EM iterations, EM converged, first centre in the replay band, Lloyd
+ * labels whose runner-up centre is within rounding (nearest_centre). */
+int two_gmm_refit_record(int32_t n_terms, const int64_t* term_sample_off, const double* delays,
+                         const int32_t* counts, uint32_t seed_select, const uint32_t* rng_skip,
+                         double* mix_out, int32_t* n_selected_out, int32_t* max_n_out, double* bic_out,
+                         int32_t* rec_out) {
   for (int t = 0; t < n_terms; ++t) {
     int mx = 0;
     int k = refit_term(delays + term_sample_off[t], counts[t], seed_select, rng_skip ? rng_skip[t] : 0u,
-                       mix_out + (size_t)t * TW_MIX_REC, &mx);
+                       mix_out + (size_t)t * TW_MIX_REC, &mx, bic_out ? bic_out + (size_t)t * TW_GMM_MAX_COMP : NULL,
+                       rec_out ? rec_out + (size_t)t * (TW_GMM_MAX_COMP + 1) * TW_GMM_REC_FIELDS : NULL);
     if (n_selected_out) n_selected_out[t] = k;
     if (max_n_out) max_n_out[t] = mx;
   }
@@ -371,7 +429,9 @@ int two_debug_kmeans_labels(const double* x, int n, int k, uint32_t seed, uint32
   double* work = (double*)malloc(sizeof(double) * (size_t)n * 4);
   mt_t rng; mt_seed(&rng, seed);
   for (uint32_t q = 0; q < skip; ++q) (void)mt_random_sample(&rng);
-  kmeans_labels(x, n, k, &rng, labels, work);
+  fitrec_t fr;
+  memset(fr, 0, sizeof fr);
+  kmeans_labels(x, n, k, &rng, labels, work, fr);
   free(work);
   return 0;
 }

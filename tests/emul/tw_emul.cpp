@@ -474,3 +474,8 @@ extern "C" int twe_skip_assess_problem(const tw_batch* b, int p, const tw_skip_d
       score, code, top2 ? margin : nullptr, prob_sum, prob_count);
   return TW_OK;
 }
+
+// first_centre (the refit's first k-means++ centre) of every (u[i], n[i])
+extern "C" void twe_first_centre(int64_t m, const double* u, const int32_t* n, int32_t* out) {
+  for (int64_t i = 0; i < m; ++i) out[i] = first_centre(u[i], n[i]);
+}

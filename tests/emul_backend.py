@@ -219,3 +219,12 @@ def conf_exp(d):
 def conf_log(x):
     """tw_core.cuh's conf_log of every element of x, on the CPU."""
     return _elementwise("twe_conf_log", x)
+
+
+def first_centre(u, n):
+    """tw_core.cuh's first_centre (the refit's first k-means++ centre) of every (u, n) pair, on the CPU."""
+    u, n = np.broadcast_arrays(np.asarray(u, np.float64), np.asarray(n, np.int32))
+    u, n = np.ascontiguousarray(u).reshape(-1), np.ascontiguousarray(n).reshape(-1)
+    out = np.zeros(len(u), np.int32)
+    lib().twe_first_centre(C.c_int64(len(u)), _ptr(u), _ptr(n), _ptr(out))
+    return out

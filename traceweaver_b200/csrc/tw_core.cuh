@@ -64,6 +64,43 @@ TW_HD int lowest_bit(uint32_t m) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// Refit (tw_gmm.cu): the first k-means++ centre, RandomState.choice(n, p = np.full(n, 1/n)) for the
+// draw u in [0, 1).
+// ---------------------------------------------------------------------------------------------
+// NumPy returns searchsorted(cdf, u, 'right') with cdf = cumsum(p) / cumsum(p)[-1], p = fl(1/n) and the
+// cumulative sum taken sequentially.  That index is floor(u n) unless u n lies within the error of
+// n cdf_i against i + 1; there the sequential sum is replayed.  With eps = 2^-53 and in units of u n, for
+// 0 <= i < n:
+//   fl(1/n) = (1 + d) / n, |d| <= eps, taken i + 1 times:              (i + 1) eps         <= n eps
+//   the i additions, each rounded to eps of a partial sum <= (j + 1)/n: (i + 1)(i + 2)/2 eps <= n (n + 1)/2 eps
+//   division by cdf_{n-1} = 1 + e, |e| <= (n + 3)/2 eps (the two lines above at i = n - 1, over n):
+//                                                                       (i + 1)(n + 3)/2 eps <= n (n + 3)/2 eps
+//   rounding of that quotient and of u n:                                                  2 n eps
+// in all (n^2 + 5n) eps to first order.  The threshold doubles it, 2^-52 n (n + 5), which also covers the
+// second-order terms while it is below 1/2; above that (n > 4.7e7) every u replays, so the rule holds for
+// every n <= INT32_MAX.  1e-6 stays as a floor: up to n ~ 67 000 nothing changes against the fixed 1e-6
+// of earlier builds; there the first-order bound is at most 5e-7 (the drift NumPy actually shows is about a
+// tenth of the bound).  A replay is two serial passes of n additions on one warp, once per fit whose draw
+// falls in the band: a share 2^-51 n (n + 5) of the draws, 4 % at n = 1e7 and every draw above 4.7e7.  A replay returns NumPy's index wherever it runs,
+// so widening the threshold only replaces floor(u n) where floor(u n) could be wrong.
+TW_HD int first_centre(double u, int n) {
+  const double un = dmul(u, (double)n);
+  int id = (int)un;
+  const double bound = fmax(1e-6, dmul(dmul((double)n, dadd((double)n, 5.0)), 0x1p-52));
+  if (fabs(dsub(un, rint(un))) < bound) {
+    const double p = ddiv(1.0, (double)n);
+    double last = 0.0, c = 0.0;
+    for (int i = 0; i < n; ++i) last = dadd(last, p);
+    id = n - 1;
+    for (int i = 0; i < n; ++i) {
+      c = dadd(c, p);
+      if (ddiv(c, last) > u) { id = i; break; }
+    }
+  }
+  return id > n - 1 ? n - 1 : id;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Likelihood terms: GetEpPairCost, V1:117-139.
 // ---------------------------------------------------------------------------------------------
 

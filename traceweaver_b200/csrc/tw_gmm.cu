@@ -140,22 +140,8 @@ __device__ __forceinline__ void seed_centres(const double* __restrict__ x, int n
   TW_GPHASE_BEGIN;
 #pragma unroll
   for (int j = 0; j < KC; ++j) cen[j] = 0.0;
-  // ---- k-means++ seeding.  First centre: RandomState.choice(n, p=1/n) = searchsorted(cdf, u,
-  // 'right') with cdf_i = (i+1 sequential adds of 1/n)/cdf_{n-1}: floor(u*n) unless u*n sits
-  // within rounding of an integer, in which case the sequential sum is replayed exactly.
-  {
-    double u = draws[0];
-    double un = dmul(u, (double)n);
-    int id = (int)un;
-    if (fabs(dsub(un, rint(un))) < 1e-6) {
-      double p = 1.0 / (double)n, last = 0.0, c = 0.0;
-      for (int i = 0; i < n; ++i) last = dadd(last, p);
-      id = n - 1;
-      for (int i = 0; i < n; ++i) { c = dadd(c, p); if (c / last > u) { id = i; break; } }
-    }
-    if (id > n - 1) id = n - 1;
-    cen[0] = dsub(x[id], mean);
-  }
+  // ---- k-means++ seeding.  First centre: RandomState.choice(n, p=1/n) (first_centre, tw_core.cuh).
+  cen[0] = dsub(x[first_centre(draws[0], n)], mean);
   const int trials = trials_for_k(k);
   double pot = 0.0;
   {
