@@ -59,7 +59,8 @@ class EmulBatch(OracleBatch):
                 W = 64
                 _check(lib().twe_score_problem(C.byref(self.struct), p, C.byref(prm) if have else None,
                                                C.byref(out), W, C.byref(ov), *self._paths()), "emul.score")
-                assert not ov.value
+                if ov.value:  # a feasible candidate at offset >= 2048: what the redo kernel reports
+                    raise _abi.TwError(_abi.TW_ERR_RANGE_LIMIT, "emul.score")
             self.overflow.append(W)
         return res
 

@@ -113,9 +113,13 @@ class BatchSolver:
 
         strict=False: a service that runs into a search limit of the engine (TW_ERR_MWIS_LIMIT: more
         than 2 M branch-and-bound nodes in one window) no longer fails the whole call: the other
-        services' results are returned, out["counters"][p, 3] holds the status of service p (0 = ok;
-        the in-spans of a failed service after the failing window stay unassigned) and
-        out["failed_services"] lists the failed ones.  Anything else still raises."""
+        services' results are returned, out["counters"][p, 3] holds the status of service p (0 = ok)
+        and out["failed_services"] lists the failed ones.  A service counts as failed when either pass
+        hit the limit: one whose first pass alone did is reported although its returned assignment may
+        be complete (the refit between the passes saw only what the first pass assigned).  A failed
+        service is stitched in units between strong cuts (DESIGN.md §8): its in-spans from the failing
+        window to the end of that unit stay unassigned; those before the window and in its later units
+        are stitched as usual.  Anything else still raises, TW_ERR_RANGE_LIMIT included."""
         dev = self.engine.device
         self._flip ^= 1
         single = truth_assign is not None or term_order is not None

@@ -15,6 +15,7 @@
 using namespace tw;
 
 static thread_local std::string g_last_error;
+static constexpr long long kDefaultNodeLimit = 2000000LL;
 
 static int fail(int code, const char* fmt, const char* a = "", const char* b2 = "") {
   char buf[512];
@@ -157,7 +158,7 @@ struct tw_engine {
   DevBuf<int32_t> prob_status;
   DevBuf<double> scaled_params;
   int64_t n_gauss_rec = 0;
-  long long node_limit = 2000000LL;   // exact MWIS search nodes per window before TW_ERR_MWIS_LIMIT
+  long long node_limit = kDefaultNodeLimit;   // exact MWIS search nodes per window before TW_ERR_MWIS_LIMIT
   // refit scratch (allocated on first tw_gmm_refit after bind)
   static constexpr int kStreamLen = 16384;
   DevBuf<int32_t> gmm_max_n;
@@ -974,6 +975,16 @@ int tw_debug_stitch_grid(tw_engine* eng, int blocks) {
   if (blocks > eng->stitch_blocks_max) return fail(TW_ERR_INVALID, "tw_debug_stitch_grid: more blocks than the bind sized");
   eng->stitch_blocks = blocks > 0 ? blocks : eng->stitch_blocks_max;
   return eng->stitch_blocks;
+}
+
+// Test hook, not part of the ABI header: exact MWIS search nodes per window before TW_ERR_MWIS_LIMIT
+// (checked by the priced search only, which components reach when the plain search runs out of its
+// budget; the small-window search takes no limit); n <= 0 restores the default of 2 000 000.  Returns the
+// limit now in effect.
+long long tw_debug_node_limit(tw_engine* eng, long long n) {
+  if (!eng) return fail(TW_ERR_INVALID, "tw_debug_node_limit: NULL engine");
+  eng->node_limit = n > 0 ? n : kDefaultNodeLimit;
+  return eng->node_limit;
 }
 
 int tw_score_assignments(tw_engine* eng, const tw_params* params, const int32_t* assign, const tw_score_out* final_topk,

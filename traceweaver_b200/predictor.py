@@ -56,6 +56,9 @@ def solve_bound(eng: Engine, seed_select=10, truth_assign=None, term_order=None,
     if after_score is not None:
         after_score(top)
     r1 = eng.stitch(p1, sc["cut"], undeleted=top)  # iteration 1
+    # the status column: a service that hit a search limit in either pass (counters[p, 3] < 0 and the
+    # engine's error flag; the last pass alone would hide a first-pass failure)
+    r1["counters"][:, 3] = r1["counters"][:, 3].minimum(r0["counters"][:, 3])
     n_cand = r0["n_cand"] + r1["n_cand"]          # per_span_candidates accumulates over iterations
     lik = eng.score_assignments(p1, r1["assign"], final_topk=top) if want_likelihood else None
     if check:
