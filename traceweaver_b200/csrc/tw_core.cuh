@@ -1070,6 +1070,28 @@ TW_HD_NOINLINE inline void assignment_solve(const WB& wb, const int* member, int
   }
 }
 
+// The tuple position whose assignment relaxation prices the branch and bound of a component (members
+// member[0 .. m), in window order): the callee with the fewest distinct spans among the candidates,
+// where the in-spans compete most; the lowest position on a tie.
+template <class WB>
+TW_HD int relaxation_position(const WB& wb, const int* member, int m, int E) {
+  int pos = 0, fewest = 0x7fffffff;
+  for (int e = 0; e < E; ++e) {
+    int distinct = 0;
+    for (int l = 0; l < m; ++l)
+      for (int r = 0; r < wb.cnt[member[l]]; ++r) {
+        const int sp = wb.at(member[l], r, e);
+        bool seen = false;
+        for (int l2 = 0; l2 <= l && !seen; ++l2)
+          for (int r2 = 0; r2 < (l2 < l ? wb.cnt[member[l2]] : r) && !seen; ++r2)
+            seen = wb.at(member[l2], r2, e) == sp;
+        distinct += !seen;
+      }
+    if (distinct < fewest) { fewest = distinct; pos = e; }
+  }
+  return pos;
+}
+
 // Solves the window; wb.adj must be filled.  Returns the number of search nodes, or -1 when
 // node_limit is exceeded (TW_ERR_MWIS_LIMIT).
 // `deferred` (device callers): components whose plain search ran out of its budget are not searched
@@ -1211,21 +1233,7 @@ TW_HD_NOINLINE inline long long mwis_solve(WB& wb, int E, int nw, long long node
     double remp[TW_WINDOW_CAP + 1], lam[TW_WINDOW_CAP + 1];
     const bool priced = m >= kMwisPricedMin;
     if (priced) {
-      int pos = 0, fewest = 0x7fffffff;           // the callee with the fewest distinct spans: most competition
-      for (int e = 0; e < E; ++e) {
-        int distinct = 0;
-        for (int l = 0; l < m; ++l)
-          for (int r = 0; r < wb.cnt[member[l]]; ++r) {
-            const int sp = wb.at(member[l], r, e);
-            bool seen = false;
-            for (int l2 = 0; l2 <= l && !seen; ++l2)
-              for (int r2 = 0; r2 < (l2 < l ? wb.cnt[member[l2]] : r) && !seen; ++r2)
-                seen = wb.at(member[l2], r2, e) == sp;
-            distinct += !seen;
-          }
-        if (distinct < fewest) { fewest = distinct; pos = e; }
-      }
-      assignment_solve(wb, member, m, pos, nullptr, price, &lam[0]);
+      assignment_solve(wb, member, m, relaxation_position(wb, member, m, E), nullptr, price, &lam[0]);
       nodes += m;
     } else {
       lam[0] = 0.0;
@@ -1442,12 +1450,14 @@ struct SmallBest {
 //   visit i, cut[i]                    -> window ended at i-1 (seen here as look-ahead), count = 0
 //   visit i, else current_count == 30  -> window ends at i, count = 0
 // A window that starts at a perfect cut can hold 31 in-spans (the count restarts at 0 there,
-// at 1 after a size cut): TW_WINDOW_CAP.
+// at 1 after a size cut): TW_WINDOW_CAP.  `cut` is the flag array, or any type whose cut[q] reads
+// flag q (the stitch kernel's register copy of the flags ahead of the window).
 // ---------------------------------------------------------------------------------------------
 struct WindowCursor {
   int count;
   TW_HD void init() { count = 1; }
-  TW_HD bool ends_at(int i, int n, const uint8_t* cut) {
+  template <class Cut>
+  TW_HD bool ends_at(int i, int n, Cut cut) {
     if (i == n - 1) return i != 0;
     bool end = false;
     if (i != 0) {

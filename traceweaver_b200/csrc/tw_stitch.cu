@@ -178,7 +178,7 @@ __device__ __noinline__ long long mwis_component_warp(PackedWindowBuf& wb, int E
       if (l == lane) kmine = k;
     }
   }
-  // ---- prices: lane 0 solves the relaxation (callee with the fewest distinct spans)
+  // ---- prices: lane 0 solves the relaxation (relaxation_position: the callee with the fewest distinct spans)
   double lam0 = 0.0;
   if (lane == 0) {
     int member[TW_WINDOW_CAP];
@@ -186,21 +186,8 @@ __device__ __noinline__ long long mwis_component_warp(PackedWindowBuf& wb, int E
       uint32_t c = comp;
       for (int l = 0; l < m; ++l) { member[l] = __ffs(c) - 1; c &= c - 1u; }
     }
-    int pos = 0, fewest = 0x7fffffff;
-    for (int e = 0; e < E; ++e) {
-      int distinct = 0;
-      for (int l = 0; l < m; ++l)
-        for (int r = 0; r < wb.cnt[member[l]]; ++r) {
-          const int sp = wb.at(member[l], r, e);
-          bool seen = false;
-          for (int l2 = 0; l2 <= l && !seen; ++l2)
-            for (int r2 = 0; r2 < (l2 < l ? wb.cnt[member[l2]] : r) && !seen; ++r2)
-              seen = wb.at(member[l2], r2, e) == sp;
-          distinct += !seen;
-        }
-      if (distinct < fewest) { fewest = distinct; pos = e; }
-    }
-    assignment_solve(wb, member, m, pos, nullptr, reinterpret_cast<double(*)[TW_K]>(price), &lam0);
+    assignment_solve(wb, member, m, relaxation_position(wb, member, m, E), nullptr,
+                     reinterpret_cast<double(*)[TW_K]>(price), &lam0);
   }
   __syncwarp();
   lam0 = __shfl_sync(kAll, lam0, 0);
@@ -320,10 +307,9 @@ __device__ __noinline__ void stitch_search_lanes(const ProbView& v, PackedWindow
   auto is_taken = [&](int e, int o) {   // volatile: bits are set by other lanes with atomics
     return (reinterpret_cast<volatile const uint32_t*>(tk_base[e])[o >> 5] >> (o & 31)) & 1u;
   };
-  const bool active = todo, fast = false;
   int lo[TW_MAX_E], r[TW_MAX_E], lo_abs[TW_MAX_E];
   int tsize = 0;
-  if (active && !fast) {
+  if (todo) {
     for (int e = 0; e < E; ++e) {
       lo[e] = lower_bound(w[e].s, w[e].n, in_s);
       lo_abs[e] = lo[e];
@@ -344,7 +330,7 @@ __device__ __noinline__ void stitch_search_lanes(const ProbView& v, PackedWindow
       store_topk_row(tk, E, out.topk_score + gi * TW_K, out.topk_idx + TW_K * (v.tuple_off + (int64_t)i * E),
                      out.topk_cnt + gi);
   };
-  bool pending = active;
+  bool pending = todo;
   // ---- heavy in-spans (thousands of candidate combinations), one at a time by the WHOLE warp:
   // the owner lays out its term tables, all lanes evaluate the slots, then the lanes take the
   // combinations lane, lane + 32, ... (ascending combination index = depth-first leaf order), keep
@@ -509,6 +495,14 @@ __device__ __noinline__ long long stitch_mwis_large(PackedWindowBuf& wb, StitchT
   }
   return nodes;
 }
+
+// Cut flags ws .. ws + 63 in registers, as WindowCursor::ends_at reads them: a window spans <= 31
+// in-spans and looks one ahead.
+struct CutBits {
+  unsigned long long bits;
+  int ws;
+  __device__ int operator[](int q) const { return (int)((bits >> (q - ws)) & 1ull); }
+};
 
 // One UNIT of the stitch by one warp: in-spans [u0, u1) of service p (u1 < 0: to the end of the service).
 __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& prm, const uint8_t* __restrict__ cut_all,
@@ -680,26 +674,10 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
     // ---- window extent (uniform across the warp)
     int we = ws;
     {
-      // cut[ws .. ws + 63] in registers; a window spans <= 31 in-spans and looks one ahead
       const unsigned c0 = __ballot_sync(0xffffffffu, ws + lane < n && cut[ws + lane] != 0);
       const unsigned c1 = __ballot_sync(0xffffffffu, ws + 32 + lane < n && cut[ws + 32 + lane] != 0);
-      const unsigned long long cm = ((unsigned long long)c1 << 32) | c0;
-      auto cutbit = [&](int q) { return (int)((cm >> (q - ws)) & 1ull); };
-      while (true) {   // WindowCursor::ends_at on the register copy
-        bool end;
-        if (we == n - 1) end = we != 0;
-        else {
-          end = false;
-          if (we != 0) {
-            if (cutbit(we)) wc.count = 0;
-            else if (wc.count == TW_MAX_WINDOW) { wc.count = 0; end = true; }
-          }
-          wc.count += 1;
-          if (cutbit(we + 1)) end = true;
-        }
-        if (end || we >= n - 1) break;
-        ++we;
-      }
+      const CutBits cb{((unsigned long long)c1 << 32) | c0, ws};
+      while (!wc.ends_at(we, n, cb) && we < n - 1) ++we;
     }
     const int nw = we - ws + 1;
     if (nw > TW_WINDOW_CAP) { rc = TW_ERR_INVALID; break; }
@@ -711,9 +689,6 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
     const bool active = lane < nw;
     const int i = ws + (active ? lane : 0);
     const int64_t in_s = v.is[i], in_e = v.ie[i];
-    auto is_taken = [&](int e, int o) {   // volatile: bits are set by other lanes with atomics
-      return (reinterpret_cast<volatile const uint32_t*>(tk_base[e])[o >> 5] >> (o & 31)) & 1u;
-    };
     // ---- fast path: none of the in-span's candidates (the spans of its feasible tuples on the
     // undeleted lists) has been taken => the undeleted top-K list IS FindTopKAssignments(out_copy)
     bool fast = false;
