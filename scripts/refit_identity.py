@@ -1,6 +1,6 @@
 """Bit-level record of the GMM refit, to compare two builds of the library.
 
-    TW_SO=path/to/libtw_b200.so python scripts/refit_identity.py dump OUT.npz
+    TW_B200_SO=path/to/libtw_b200.so python scripts/refit_identity.py dump OUT.npz
     python scripts/refit_identity.py compare A.npz B.npz
 
 dump: pass 0, the delays of its assignments and tw_gmm_refit(want_selected) on bench.py's streams
@@ -19,9 +19,6 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def dump(out_path):
-    from traceweaver_b200 import _lib
-    if os.environ.get("TW_SO"):
-        _lib.SO_PATH = os.environ["TW_SO"]
     import torch
     from golden_util import Golden, GOLDEN_DIR
     from traceweaver_b200 import shard

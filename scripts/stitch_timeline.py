@@ -1,16 +1,16 @@
-"""Busy warp slots of k_stitch over time in both passes (library built with -DTW_STITCH_TIMELINE:
-`python -c "from traceweaver_b200.csrc import build; build.build_variant('timeline', ['TW_STITCH_TIMELINE'])"`).
+"""Busy warp slots of k_stitch over time in both passes, read from the timeline build of the library:
+
+    python -m traceweaver_b200.csrc.build --timeline
+    TW_B200_SO=traceweaver_b200/libtw_b200_timeline.so python scripts/stitch_timeline.py [n_services] [hotel|media|alibaba]
+
 Every warp records the %globaltimer at the start of its first unit and the end of its last one; the
 script prints the mean number of busy warps per tenth of the kernel and the share of the kernel's
-duration during which fewer than half of the resident warp slots (SMs x 28) are busy.
-Usage: python scripts/stitch_timeline.py [n_services] [hotel|media|alibaba]"""
+duration during which fewer than half of the resident warp slots (SMs x 28) are busy."""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
-from traceweaver_b200 import _lib
-_lib.SO_PATH = os.environ.get("TW_B200_SO") or os.path.join(os.path.dirname(_lib.SO_PATH), "libtw_b200_timeline.so")
 import torch
-from traceweaver_b200 import shard
+from traceweaver_b200 import _lib, shard
 from traceweaver_b200.batch import build_batch_from_blocks
 from traceweaver_b200.engine import Engine
 
@@ -18,14 +18,16 @@ RESIDENT_WARPS_PER_SM = 28      # tw_kernels.cuh: kStitchWarps * kStitchBlocksPe
 CAP = 1 << 18                   # tw_stitch.cu: kTimelineCap
 BINS = 10
 
+lib = _lib.load()
+if not hasattr(lib, "tw_debug_stitch_timeline"):
+    sys.exit(f"{_lib.SO_PATH} has no stitch timeline: build it with --timeline and name it in TW_B200_SO")
+lib.tw_debug_stitch_timeline.argtypes = [C.c_void_p, C.c_int, C.c_int]
 S = int(sys.argv[1]) if len(sys.argv) > 1 else 8192
 wl = sys.argv[2] if len(sys.argv) > 2 else "hotel"
 hb = build_batch_from_blocks(shard.generate_slice(shard.stream_spec(wl, S, 1000, 10), 0, S))
 eng = Engine(0); eng.bind(hb); eng.prepare()
 p0 = eng.params_pass0(); sc = eng.score(p0, want_used=True); r0 = eng.stitch(p0, sc["cut"], undeleted=sc)
 p1 = eng.gmm_refit(*eng.delays(r0["assign"])); top = eng.score(p1, want_used=True)
-lib = _lib.load()
-lib.tw_debug_stitch_timeline.argtypes = [C.c_void_p, C.c_int, C.c_int]
 buf = np.zeros(3 * CAP, np.uint64)
 slots = torch.cuda.get_device_properties(0).multi_processor_count * RESIDENT_WARPS_PER_SM
 

@@ -1,11 +1,8 @@
-"""Time only the refit with alternative builds of the library (TW_SO env var)."""
+"""Time only the refit, of the library TW_B200_SO names (default: the in-tree build)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from traceweaver_b200 import _lib
-if os.environ.get("TW_SO"):
-    _lib.SO_PATH = os.environ["TW_SO"]
 import torch
-from traceweaver_b200 import synth
+from traceweaver_b200 import _lib, synth
 from traceweaver_b200.batch import build_batch_from_blocks
 from traceweaver_b200.engine import Engine
 blocks = synth.hotel_stream(8192, 1000, seed=10); hb = build_batch_from_blocks(blocks)
@@ -18,4 +15,4 @@ a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True
 a.record()
 for _ in range(3): eng.gmm_refit(d, c)
 b.record(); torch.cuda.synchronize()
-print(os.environ.get("TW_SO", "default"), "gmm_refit ms", a.elapsed_time(b) / 3)
+print(_lib.SO_PATH, "gmm_refit ms", a.elapsed_time(b) / 3)

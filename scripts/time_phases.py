@@ -3,9 +3,6 @@ Usage: python scripts/time_phases.py [n_services] [n_in]"""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
-from traceweaver_b200 import _lib
-if os.environ.get("TW_SO"):
-    _lib.SO_PATH = os.environ["TW_SO"]
 from traceweaver_b200 import synth
 from traceweaver_b200.batch import build_batch_from_blocks
 from traceweaver_b200.engine import Engine

@@ -8,7 +8,7 @@ import os
 from . import _abi
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# TW_B200_SO: developer override to load a measurement variant of the library (csrc/build.py: build_variant)
+# TW_B200_SO: developer override to load a measurement build of the library (csrc/build.py: --prof, --timeline)
 SO_PATH = os.environ.get("TW_B200_SO") or os.path.join(_HERE, "libtw_b200.so")
 _LIB = None
 

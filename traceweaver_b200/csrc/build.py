@@ -1,8 +1,13 @@
 """Build libtw_b200.so (hand-written sm_90a CUDA for the H100 + C ABI) in-tree with nvcc.
 
-    python -m traceweaver_b200.csrc.build [--force] [--verbose]
+    python -m traceweaver_b200.csrc.build [--force] [--verbose] [--prof | --timeline]
 
-nvcc cross-compiles without a GPU; the .so is a build product and stays out of git."""
+--prof builds libtw_b200_prof.so, with the phase counters of the scoring, stitch and refit kernels
+(TW_PROFILE_PHASES; scripts/phase_profile.py reads them); --timeline builds libtw_b200_timeline.so,
+with the stitch kernel's warp timeline (TW_STITCH_TIMELINE; scripts/stitch_timeline.py).  The product
+never loads these measurement builds: a script loads one when TW_B200_SO names it.
+
+nvcc cross-compiles without a GPU; the .so files are build products and stay out of git."""
 import glob
 import os
 import subprocess
@@ -10,7 +15,6 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
-OUT = os.path.join(PKG, "libtw_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-shared", "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-Xptxas", "-v",
@@ -21,55 +25,39 @@ def sources():
     return sorted(glob.glob(os.path.join(HERE, "*.cu")))
 
 
-def stale():
-    if not os.path.exists(OUT):
+def stale(out):
+    if not os.path.exists(out):
         return True
-    t = os.path.getmtime(OUT)
+    t = os.path.getmtime(out)
     deps = sources() + glob.glob(os.path.join(HERE, "*.cuh")) + \
         [os.path.join(PKG, "..", "include", "traceweaver_b200.h"), os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False):
-    if not force and not stale():
-        return OUT
-    cmd = [NVCC] + FLAGS + ["-o", OUT] + sources()
+def build(force=False, verbose=False, defines=(), name=None):
+    """libtw_b200.so, or libtw_b200_<name>.so compiled with -D<d> for every d in `defines`."""
+    if defines and not name:
+        raise ValueError("a build with extra defines needs a name of its own")
+    suffix = f"_{name}" if name else ""
+    out = os.path.join(PKG, f"libtw_b200{suffix}.so")
+    if not force and not stale(out):
+        return out
+    cmd = [NVCC] + FLAGS + [f"-D{d}" for d in defines] + ["-o", out] + sources()
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    log = os.path.join(HERE, "build.log")
+    log = os.path.join(HERE, f"build{suffix}.log")
     with open(log, "w") as f:
         f.write(" ".join(cmd) + "\n" + res.stdout)
     if verbose or res.returncode != 0:
         print(res.stdout)
     if res.returncode != 0:
         raise RuntimeError(f"nvcc failed ({res.returncode}); see {log}")
-    return OUT
-
-
-def build_profiling():
-    """libtw_b200_prof.so: the same sources with -DTW_PROFILE_PHASES (clock64 phase timers inside the
-    scoring / stitch / refit kernels; scripts/*_phase_profile.py read them).  Never used by the product."""
-    out = os.path.join(PKG, "libtw_b200_prof.so")
-    cmd = [NVCC] + FLAGS + ["-DTW_PROFILE_PHASES", "-o", out] + sources()
-    res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    if res.returncode != 0:
-        print(res.stdout)
-        raise RuntimeError("nvcc failed (profiling build)")
-    return out
-
-
-def build_variant(name, defines):
-    """libtw_b200_<name>.so with extra -D flags: measurement variants (scripts/*), never used by the product."""
-    out = os.path.join(PKG, f"libtw_b200_{name}.so")
-    cmd = [NVCC] + FLAGS + [f"-D{d}" for d in defines] + ["-o", out] + sources()
-    res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    if res.returncode != 0:
-        print(res.stdout)
-        raise RuntimeError(f"nvcc failed (variant {name})")
     return out
 
 
 if __name__ == "__main__":
+    name, defines = None, ()
     if "--prof" in sys.argv:
-        print(build_profiling())
-    else:
-        print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv))
+        name, defines = "prof", ("TW_PROFILE_PHASES",)
+    elif "--timeline" in sys.argv:
+        name, defines = "timeline", ("TW_STITCH_TIMELINE",)
+    print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv, defines=defines, name=name))

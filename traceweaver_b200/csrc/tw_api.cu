@@ -987,6 +987,24 @@ long long tw_debug_node_limit(tw_engine* eng, long long n) {
   return eng->node_limit;
 }
 
+#ifdef TW_PROFILE_PHASES
+// Measurement hook of the profiling build, not part of the ABI header: copies the first n (<= kPhaseSlots)
+// phase counters of kernel 0 (scoring), 1 (stitch) or 2 (refit) to `out`, then zeroes them all if `reset`.
+int tw_debug_phases(int kernel, unsigned long long* out, int n, int reset) {
+  cudaError_t (*const bank_of[])(void**) = {score_phase_bank, stitch_phase_bank, gmm_phase_bank};
+  if (kernel < 0 || kernel > 2 || !out || n < 0 || n > kPhaseSlots)
+    return fail(TW_ERR_INVALID, "tw_debug_phases: bad argument");
+  void* bank = nullptr;
+  CU(bank_of[kernel](&bank));
+  CU(cudaMemcpy(out, bank, n * sizeof *out, cudaMemcpyDeviceToHost));
+  if (reset) {
+    CU(cudaMemset(bank, 0, kPhaseSlots * sizeof *out));
+    CU(cudaDeviceSynchronize());
+  }
+  return TW_OK;
+}
+#endif
+
 int tw_score_assignments(tw_engine* eng, const tw_params* params, const int32_t* assign, const tw_score_out* final_topk,
                          double* score_out, uint8_t* code_out, double* margin_out, double* prob_sum_out,
                          int32_t* prob_count_out, void* stream) {

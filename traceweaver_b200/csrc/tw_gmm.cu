@@ -34,29 +34,11 @@ constexpr int KC = TW_GMM_MAX_COMP;
 constexpr unsigned kFull = 0xffffffffu;
 constexpr int kLloydLabelN = 1024;   // longest sample list whose Lloyd labels stay in shared memory
 
-// optional phase timers (build with -DTW_PROFILE_PHASES; scripts/phase_profile.py reads them):
-// cycles in seeding / Lloyd / initial M-step / EM / scoring, then Lloyd and EM iteration counts, fits
+// phase counters (tw_kernels.cuh): cycles in seeding / Lloyd / initial M-step / EM / scoring in 0-4,
+// then Lloyd iterations, EM iterations and fits in 5-7
+TW_PHASE_BANK(g_gmm_phase);
 #ifdef TW_PROFILE_PHASES
-__device__ unsigned long long g_gmm_phase[16];
-#define TW_GPHASE_BEGIN long long _gp_t0 = clock64()
-#define TW_GPHASE_RESET _gp_t0 = clock64()
-#define TW_GPHASE(k)                                                               \
-  do {                                                                             \
-    if ((threadIdx.x & 31) == 0) {                                                 \
-      long long _now = clock64();                                                  \
-      atomicAdd(&g_gmm_phase[k], (unsigned long long)(_now - _gp_t0));             \
-      _gp_t0 = _now;                                                               \
-    }                                                                              \
-  } while (0)
-#define TW_GCOUNT(k, v)                                                            \
-  do {                                                                             \
-    if ((threadIdx.x & 31) == 0) atomicAdd(&g_gmm_phase[k], (unsigned long long)(v)); \
-  } while (0)
-#else
-#define TW_GPHASE_BEGIN do { } while (0)
-#define TW_GPHASE_RESET do { } while (0)
-#define TW_GPHASE(k) do { } while (0)
-#define TW_GCOUNT(k, v) do { } while (0)
+cudaError_t gmm_phase_bank(void** bank) { return cudaGetSymbolAddress(bank, g_gmm_phase); }
 #endif
 
 // Work of the EM sweeps (always on; one atomic per fit): sample-component evaluations of the E+M sweep.
@@ -137,7 +119,7 @@ __device__ __forceinline__ void seed_centres(const double* __restrict__ x, int n
                                              const double* __restrict__ draws, double* cen) {
   const int lane = threadIdx.x & 31;
   const int k = K;
-  TW_GPHASE_BEGIN;
+  TW_PHASE_START(phase_t0);
 #pragma unroll
   for (int j = 0; j < KC; ++j) cen[j] = 0.0;
   // ---- k-means++ seeding.  First centre: RandomState.choice(n, p=1/n) (first_centre, tw_core.cuh).
@@ -199,7 +181,7 @@ __device__ __forceinline__ void seed_centres(const double* __restrict__ x, int n
     cen[ci] = cc[best];
     pot = bp;
   }
-  TW_GPHASE(0);
+  TW_PHASE(g_gmm_phase, phase_t0, 0);
 }
 
 // Lloyd iterations from the seeded centres: cen[] in, the centres that define the final labels_ out.
@@ -209,7 +191,7 @@ __device__ __forceinline__ void lloyd_centres(const double* __restrict__ x, int 
                                               const double* cen_in, double* cen_out, unsigned char* labs) {
   const int lane = threadIdx.x & 31;
   const int k = K;
-  TW_GPHASE_BEGIN;
+  TW_PHASE_START(phase_t0);
   double cen[KC];
 #pragma unroll
   for (int j = 0; j < KC; ++j) cen[j] = cen_in[j];
@@ -321,7 +303,7 @@ __device__ __forceinline__ void lloyd_centres(const double* __restrict__ x, int 
       }
     }
     have_prev = true;
-    TW_GCOUNT(5, 1);
+    TW_COUNT(g_gmm_phase, 5, 1);
     if (!changed) { strict = true; break; }
     if (shift_tot <= tol) break;
   }
@@ -329,7 +311,7 @@ __device__ __forceinline__ void lloyd_centres(const double* __restrict__ x, int 
   // final update); otherwise sklearn re-runs the assignment with the final centres
 #pragma unroll
   for (int j = 0; j < KC; ++j) cen_out[j] = strict ? prev[j] : cen[j];
-  TW_GPHASE(1);
+  TW_PHASE(g_gmm_phase, phase_t0, 1);
 }
 
 // v[lane] on lanes 0..K-1, v[0] on the others: hands each of the first K lanes its component of a
@@ -436,11 +418,11 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
   const double shift = FULL ? mean : 0.0;
   double S0[KC], S1[KC], S2[KC], nk[KC], mup[KC];
   double my_nk, my_mup, my_s2;       // this lane's component (lanes 0..K-1)
-  TW_GPHASE_BEGIN;
+  TW_PHASE_START(phase_t0);
   {
     double cen2[KC];
     centre_squares<K>(cen, cen2);
-    TW_GCOUNT(7, 1);
+    TW_COUNT(g_gmm_phase, 7, 1);
 #pragma unroll
     for (int c = 0; c < KC; ++c) { S0[c] = 0.0; S1[c] = 0.0; S2[c] = 0.0; }
     sweep2(x, n, [&](double x0, double x1, bool v1, int) {
@@ -490,7 +472,7 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
     my_s2 = lane_component<K>(S2);
   }
   if (!params_from_stats<K, FULL>(f, n, my_nk, my_mup, my_s2, 0.0, shift, true)) return false;
-  TW_GPHASE(2);
+  TW_PHASE(g_gmm_phase, phase_t0, 2);
   double lower = -INFINITY;
   int em_sweeps = 0;
   for (int it = 1; it <= kEmMaxIter; ++it) {
@@ -545,12 +527,12 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
       if (lane == 0) atomicAdd(&g_gmm_em_evals, (unsigned long long)it * (unsigned long long)n * K);
       return false;
     }
-    TW_GCOUNT(6, 1);
+    TW_COUNT(g_gmm_phase, 6, 1);
     em_sweeps = it;
     if (fabs(lower - prev) < kEmTol) break;
   }
   if (lane == 0) atomicAdd(&g_gmm_em_evals, (unsigned long long)(em_sweeps + (want_score ? 1 : 0)) * (unsigned long long)n * K);
-  TW_GPHASE(3);
+  TW_PHASE(g_gmm_phase, phase_t0, 3);
   if (want_score) {
     LogSum ls;
     for (int i = lane; i < n; i += 32) {
@@ -560,7 +542,7 @@ __device__ __forceinline__ bool em_fit(const double* __restrict__ x, int n, doub
     }
     *score = wsum(ls.total()) / (double)n;
   }
-  TW_GPHASE(4);
+  TW_PHASE(g_gmm_phase, phase_t0, 4);
   return true;
 }
 
@@ -888,18 +870,6 @@ cudaError_t gmm_work_read(unsigned long long* out, bool reset) {
   }
   return e;
 }
-
-#ifdef TW_PROFILE_PHASES
-extern "C" int tw_debug_gmm_phases(unsigned long long* out16, int reset) {
-  cudaError_t e = cudaMemcpyFromSymbol(out16, g_gmm_phase, sizeof(unsigned long long) * 16);
-  if (e != cudaSuccess) return -2;
-  if (reset) {
-    unsigned long long z[16] = {0};
-    cudaMemcpyToSymbol(g_gmm_phase, z, sizeof z);
-  }
-  return 0;
-}
-#endif
 
 cudaError_t launch_gmm_prep(int n_terms, const int64_t* term_sample_off, const double* delays,
                             const int32_t* counts, int32_t* max_n, double* mean_var, cudaStream_t s,

@@ -7,15 +7,45 @@
 
 namespace tw {
 
+// ---- phase counters of the profiling build (-DTW_PROFILE_PHASES; scripts/phase_profile.py) -----------
+// The scoring, stitch and refit kernel files each keep a bank of kPhaseSlots counters, a __device__ array
+// of their own translation unit (the library is built without -rdc).  TW_PHASE adds the clock64() cycles
+// since `timer` was last set to slot k and restarts it; TW_COUNT adds v to slot k.  Lane 0 of each warp
+// does the atomicAdd.  tw_debug_phases (tw_api.cu) reads a bank through its file's accessor.  In the
+// product build the macros are empty.
+constexpr int kPhaseSlots = 24;
+#ifdef TW_PROFILE_PHASES
+#define TW_PHASE_BANK(bank) __device__ unsigned long long bank[kPhaseSlots]
+#define TW_PHASE_START(timer) long long timer = clock64()
+#define TW_PHASE(bank, timer, k)                                               \
+  do {                                                                         \
+    if ((threadIdx.x & 31) == 0) {                                             \
+      const long long _now = clock64();                                        \
+      atomicAdd(&bank[k], (unsigned long long)(_now - timer));                 \
+      timer = _now;                                                            \
+    }                                                                          \
+  } while (0)
+#define TW_COUNT(bank, k, v)                                                   \
+  do {                                                                         \
+    if ((threadIdx.x & 31) == 0) atomicAdd(&bank[k], (unsigned long long)(v)); \
+  } while (0)
+// the device address of each file's bank
+cudaError_t score_phase_bank(void** bank);       // tw_score3.cu: k_score3
+cudaError_t stitch_phase_bank(void** bank);      // tw_stitch.cu: k_stitch
+cudaError_t gmm_phase_bank(void** bank);         // tw_gmm.cu: the fit kernels
+#else
+#define TW_PHASE_BANK(bank) static_assert(true, "")   // declares nothing; the use's ';' stays valid
+#define TW_PHASE_START(timer) do { } while (0)
+#define TW_PHASE(bank, timer, k) do { } while (0)
+#define TW_COUNT(bank, k, v) do { } while (0)
+#endif
+
 // ---- score kernel geometry (tw_score.cu) ----------------------------------------------------
 constexpr int kS3Threads = 128;                  // tw_score3.cu: one CTA = one tile, one warp = 32 in-spans
 constexpr int kS3Tile = 128;                     // in-spans per tile
 constexpr int kStageSpans = 1536;                // out spans staged in shared memory per tile
 constexpr int kTblCap = 3072;                    // term-table slots of a redo CTA (tw_score.cu)
-#ifndef TW_WARP_TBL_CAP
-#define TW_WARP_TBL_CAP 256
-#endif
-constexpr int kWarpTblCap = TW_WARP_TBL_CAP;     // term-table slots per stitch warp (search path only)
+constexpr int kWarpTblCap = 256;                 // term-table slots per stitch warp (search path only)
 constexpr int kRedoCoopCombos = 256;             // redo kernel: in-spans with more combinations are scored by the whole warp
 constexpr int kStitchCoopCombos = 512;           // in-spans with more candidate combinations are searched by the whole warp
 constexpr int kTakenWords = 256;                 // taken-bitmap words a stitch warp keeps in shared memory

@@ -32,47 +32,23 @@
 //   * results leave through shared memory as coalesced 128-bit stores.
 //
 // Anything this kernel cannot do EXACTLY is not approximated: the tile is flagged and redone by
-// the sequential kernel (k_score<32,64>, tw_score.cu): more than 64 candidates of one ep in an
+// the sequential kernel (k_score, tw_score.cu): more than 64 candidates of one ep in an
 // in-span's range, more than 2^24 combinations, a slice that does not fit the staging buffer, two
 // tuples of one in-span with the same score (the reference's heap order decides), a NaN score.
 #include "tw_kernels.cuh"
 
 namespace tw {
 
-// optional phase timers / work counters (build with -DTW_PROFILE_PHASES; scripts/score_phase_profile.py)
+// phase counters (tw_kernels.cuh): cycles of phases 0-7, then slots, combinations, rounds, feasible
+// tuples, valid slots, and tiles / warps flagged for the sequential kernel in 10-17
+TW_PHASE_BANK(g_score_phase);
 #ifdef TW_PROFILE_PHASES
-__device__ unsigned long long g_score_phase[24];
-#define TW_CPHASE(k)                                                                 \
-  do {                                                                               \
-    if (lane == 0) {                                                                 \
-      long long _now = clock64();                                                    \
-      atomicAdd(&g_score_phase[k], (unsigned long long)(_now - _cp_t0));             \
-      _cp_t0 = _now;                                                                 \
-    }                                                                                \
-  } while (0)
-#define TW_CCOUNT(k, v) do { if (lane == 0) atomicAdd(&g_score_phase[k], (unsigned long long)(v)); } while (0)
-extern "C" int tw_debug_score_phases(unsigned long long* out24, int reset) {
-  cudaError_t e = cudaMemcpyFromSymbol(out24, g_score_phase, sizeof(unsigned long long) * 24);
-  if (e != cudaSuccess) return -2;
-  if (reset) {
-    unsigned long long z[24] = {0};
-    cudaMemcpyToSymbol(g_score_phase, z, sizeof z);
-  }
-  return 0;
-}
-#else
-#define TW_CPHASE(k) do { } while (0)
-#define TW_CCOUNT(k, v) do { } while (0)
+cudaError_t score_phase_bank(void** bank) { return cudaGetSymbolAddress(bank, g_score_phase); }
 #endif
 
-#ifndef TW_S3_TBL
-#define TW_S3_TBL 416          // term-table slots per warp per round
-#define TW_S3_ENT 192          // feasible tuples per warp between two flushes of the list
-#define TW_S3_PRM_TERMS 16     // likelihood records staged in shared memory (else read in place)
-#endif
-constexpr int kS3Tbl = TW_S3_TBL;
-constexpr int kS3Ent = TW_S3_ENT;
-constexpr int kS3Prm = TW_S3_PRM_TERMS * TW_MIX_REC;
+constexpr int kS3Tbl = 416;                 // term-table slots per warp per round
+constexpr int kS3Ent = 192;                 // feasible tuples per warp between two flushes of the list
+constexpr int kS3Prm = 16 * TW_MIX_REC;     // likelihood records staged in shared memory (else read in place)
 constexpr int kS3Warps = kS3Threads / 32;
 constexpr unsigned kFull = 0xffffffffu;
 constexpr int kS3MaxR = 64;                 // candidates of one ep in one in-span's range
@@ -222,9 +198,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
   using XP = typename S3Pack<E>::xp_t;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const int t = blockIdx.x;
-#ifdef TW_PROFILE_PHASES
-  long long _cp_t0 = clock64();
-#endif
+  TW_PHASE_START(phase_t0);
   if (keep_windows && overflow_flag[t]) return;      // the sequential kernel owns this tile
   const int p = tiles.tile_prob[t];
   const int i0 = tiles.tile_start[t];
@@ -247,7 +221,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
   for (int e = 0; e < E; ++e) tot += (tw[2 * e + 1] + 3) & ~1;
   if (tot > S3Smem<E>::kStage) {
     if (tid == 0 && !keep_windows) overflow_flag[t] = 1;
-    if (tid == 0) { TW_CCOUNT(15, 1); }           // staging overflow
+    if (tid == 0) { TW_COUNT(g_score_phase, 15, 1); }  // staging overflow
     return;
   }
   if (tid == 0) mbar_init(&sm.bar, 2 * E);
@@ -318,7 +292,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
   mbar_wait(&sm.bar, 0);
   __syncthreads();                                   // heads / tails / layout visible
 
-  TW_CPHASE(0);                                      // header, staging, barrier
+  TW_PHASE(g_score_phase, phase_t0, 0);              // header, staging, barrier
   // ================= from here on the warps are independent =================
   const uint32_t* magic = sm.magic;
   // sink eps: the LAST term (V1:354-355) can only fall on an ep without DAG successors, unless end
@@ -351,7 +325,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
   if (P > kS3MaxP) { anomaly = true; P = 0; }
   if (__any_sync(kFull, anomaly)) {
     if (lane == 0 && !keep_windows) overflow_flag[t] = 1;
-    TW_CCOUNT(16, 1);                                // range wider than 64 / too many combinations (per warp)
+    TW_COUNT(g_score_phase, 16, 1);                  // range wider than 64 / too many combinations (per warp)
     return;   // (with keep_windows the flag is already set: same data, same decision)
   }
   // table size: root / sink-last terms r_e, edge terms r_b * r_e
@@ -366,7 +340,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
   }
   const bool direct = tsize > kS3Tbl;        // tables do not fit: terms are evaluated per feasible tuple
 
-  TW_CPHASE(1);                                      // candidate ranges, table sizes
+  TW_PHASE(g_score_phase, phase_t0, 1);              // candidate ranges, table sizes
   // top-K of the own in-span: keys descending, 0 = empty
   unsigned long long tk0 = 0, tk1 = 0, tk2 = 0, tk3 = 0, tk4 = 0;
   XP tx0 = 0, tx1 = 0, tx2 = 0, tx3 = 0, tx4 = 0;
@@ -396,10 +370,10 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
     const int cstart = cend - cneed;
     const int total_c = __shfl_sync(kFull, cend, 31);
 
-    TW_CPHASE(2);                                    // admission
-    TW_CCOUNT(10, total_t);
-    TW_CCOUNT(11, total_c);
-    TW_CCOUNT(12, 1);
+    TW_PHASE(g_score_phase, phase_t0, 2);            // admission
+    TW_COUNT(g_score_phase, 10, total_t);
+    TW_COUNT(g_score_phase, 11, total_c);
+    TW_COUNT(g_score_phase, 12, 1);
     // ---- 1. term tables, TERM-MAJOR: for one term at a time the slots of all admitted in-spans are
     // flattened over the warp, so the term, its eps, the candidate-count fields and (mixture pass)
     // the likelihood record and its component count are warp-uniform: no per-slot term search, no
@@ -450,7 +424,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
           }
           // valid slots are compacted so that the FP64 work below runs on full warps
           const unsigned vm = __ballot_sync(kFull, valid);
-          TW_CCOUNT(14, __popc(vm));
+          TW_COUNT(g_score_phase, 14, __popc(vm));
           if (valid) {
             const int pos = nv + __popc(vm & ((1u << lane) - 1u));
             const int brel = prm.mode == TW_PARAMS_GAUSS_BATCHED ? (i0 + wid * 32 + j) / TW_PARAM_BATCH - batch0 : 0;
@@ -480,7 +454,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
     }
     __syncwarp();
 
-    TW_CPHASE(3);                                    // term tables
+    TW_PHASE(g_score_phase, phase_t0, 3);            // term tables
     // ---- 2. combinations, in chunks of the entry list
     int n_ent = 0;
     int base = 0;
@@ -537,8 +511,8 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
         n_ent += __popc(m);
       }
       __syncwarp();
-      TW_CPHASE(4);                                  // 2a feasibility
-      TW_CCOUNT(13, n_ent);
+      TW_PHASE(g_score_phase, phase_t0, 4);          // 2a feasibility
+      TW_COUNT(g_score_phase, 13, n_ent);
       // 2b. scores: sum of table entries in the reference's term order (V1:316-357)
       if (has_params) {
         for (int eb = 0; eb < n_ent; eb += 32) {
@@ -598,7 +572,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
         }
         __syncwarp();
       }
-      TW_CPHASE(5);                                  // 2b scores
+      TW_PHASE(g_score_phase, phase_t0, 5);          // 2b scores
       // 2c. per-owner segments of the list (entries are grouped by owner, in leaf order)
       ws.seg_lo[lane] = 0;
       ws.seg_hi[lane] = 0;
@@ -702,7 +676,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
         }
       }
       __syncwarp();
-      TW_CPHASE(6);                                  // 2c top-K
+      TW_PHASE(g_score_phase, phase_t0, 6);          // 2c top-K
       n_ent = 0;
       if (base >= total_c) break;
     }
@@ -710,11 +684,11 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
   }
   if (__any_sync(kFull, redo)) {
     if (lane == 0) overflow_flag[t] = 1;       // (also under keep_windows: a score tie depends on the parameters)
-    TW_CCOUNT(17, 1);                                // tie / NaN (per warp)
+    TW_COUNT(g_score_phase, 17, 1);                  // tie / NaN (per warp)
     return;
   }
 
-  TW_CPHASE(2);
+  TW_PHASE(g_score_phase, phase_t0, 2);
   // ================= results, staged through shared memory =================
   const int w0 = wid * 32;
   const int nv = min(32, cnt - w0);            // in-spans of this warp
@@ -770,7 +744,7 @@ k_score3(tw_batch b, tw_params prm, int has_params, int keep_windows, tw_score_o
     warp_copy_out(out.used_bits + 2 * tb, &ws.used[0][0][0], nv * E * kNarrowW, lane);
     if (worker) out.used_wide[g0 + lane] = 0;
   }
-  TW_CPHASE(7);                                      // results
+  TW_PHASE(g_score_phase, phase_t0, 7);              // results
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -18,21 +18,11 @@
 
 namespace tw {
 
-// optional phase timers (build with -DTW_PROFILE_PHASES; scripts/stitch_phase_profile.py reads them)
+// phase counters (tw_kernels.cuh): cycles of phases 0-8, then runs, in-spans in runs, windows, in-spans
+// in windows, slow in-spans and large-MWIS windows in 10-15
+TW_PHASE_BANK(g_stitch_phase);
 #ifdef TW_PROFILE_PHASES
-__device__ unsigned long long g_stitch_phase[16];
-#define TW_SPHASE(k)                                                                 \
-  do {                                                                               \
-    if (lane == 0) {                                                                 \
-      long long _now = clock64();                                                    \
-      atomicAdd(&g_stitch_phase[k], (unsigned long long)(_now - _sp_t0));            \
-      _sp_t0 = _now;                                                                 \
-    }                                                                                \
-  } while (0)
-#define TW_SCOUNT(k, v) do { if (lane == 0) atomicAdd(&g_stitch_phase[k], (unsigned long long)(v)); } while (0)
-#else
-#define TW_SPHASE(k) do { } while (0)
-#define TW_SCOUNT(k, v) do { } while (0)
+cudaError_t stitch_phase_bank(void** bank) { return cudaGetSymbolAddress(bank, g_stitch_phase); }
 #endif
 
 // optional warp timeline (build with -DTW_STITCH_TIMELINE; scripts/stitch_timeline.py reads it): per
@@ -511,9 +501,7 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
                                             int* __restrict__ err_flag, const StitchSlab& slab, const double* etab,
                                             int lane, int p, int u0, int u1) {
   StitchWarpSmem& sm = slab.fixed();
-#ifdef TW_PROFILE_PHASES
-  long long _sp_t0 = clock64();
-#endif
+  TW_PHASE_START(phase_t0);
   int rc = TW_OK;
   if (lane == 0) rc = load_view(b, p, sm.v);
   rc = __shfl_sync(0xffffffffu, rc, 0);
@@ -566,7 +554,7 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
   int ws = u0;
   bool skip_run = false;
   const bool can_run = tk_smem && spec.used_lo != nullptr && out.topk_score == nullptr;
-  TW_SPHASE(0);                                  // setup + defaults
+  TW_PHASE(g_stitch_phase, phase_t0, 0);         // setup + defaults
   // The per-in-span records the run / adopt paths read (maps, top-K lists, counts) were written by the
   // scoring kernel and are cold; every step of this sequential walk would otherwise wait for them one
   // dependent miss after the other.  Each lane asks for the records of in-span (ws + 32 + lane) — one
@@ -605,7 +593,7 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
       const bool single = ij < u1 && (ij == n - 1 ? ij != 0 : cut[ij + 1] != 0);
       const unsigned sm_mask = __ballot_sync(0xffffffffu, single);
       const int R = sm_mask == 0xffffffffu ? 32 : __ffs(~sm_mask) - 1;
-      TW_SPHASE(1);                              // run extent (cut flags)
+      TW_PHASE(g_stitch_phase, phase_t0, 1);     // run extent (cut flags)
       if (R >= 1) {
         const bool act = lane < R;
         const int ir = ws + (act ? lane : 0);
@@ -640,7 +628,7 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
           }
         }
         __syncwarp();
-        TW_SPHASE(2);                            // run test
+        TW_PHASE(g_stitch_phase, phase_t0, 2);   // run test
         if (all_ok) {
           int rank = -2;
           if (act) {
@@ -662,9 +650,9 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
           __syncwarp();
           wc.count = 1;
           ws += R;
-          TW_SPHASE(3);                          // run commit
-          TW_SCOUNT(10, 1);
-          TW_SCOUNT(11, R);
+          TW_PHASE(g_stitch_phase, phase_t0, 3); // run commit
+          TW_COUNT(g_stitch_phase, 10, 1);
+          TW_COUNT(g_stitch_phase, 11, R);
           continue;
         }
         skip_run = true;   // conflict: do this window the long way, then try runs again
@@ -681,9 +669,9 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
     }
     const int nw = we - ws + 1;
     if (nw > TW_WINDOW_CAP) { rc = TW_ERR_INVALID; break; }
-    TW_SPHASE(4);                                // window extent
-    TW_SCOUNT(12, 1);
-    TW_SCOUNT(13, nw);
+    TW_PHASE(g_stitch_phase, phase_t0, 4);       // window extent
+    TW_COUNT(g_stitch_phase, 12, 1);
+    TW_COUNT(g_stitch_phase, 13, nw);
 
     // ---- per-lane candidate ranges on the not-taken spans
     const bool active = lane < nw;
@@ -727,15 +715,15 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
         }
       }
     }
-    TW_SPHASE(5);                                // fast test + adopt
+    TW_PHASE(g_stitch_phase, phase_t0, 5);       // fast test + adopt
     // ---- slow path (kept out of line: the hot loop above and below stays small in the instruction cache)
     const unsigned slow_mask = __ballot_sync(0xffffffffu, active && !fast);   // (all lanes vote: the counter macro runs on lane 0 only)
-    TW_SCOUNT(14, __popc(slow_mask));
+    TW_COUNT(g_stitch_phase, 14, __popc(slow_mask));
     if (slow_mask)
       stitch_search_lanes(v, wb, tb, prm, out, tk_base, w, gauss_base, mix_base, etab, E, lane, ws, i, in_s, in_e,
                           active && !fast, batch0);
     __syncwarp();
-    TW_SPHASE(6);                                // slow path
+    TW_PHASE(g_stitch_phase, phase_t0, 6);       // slow path
     // ---- stitch the window (V3:1192-1219)
     long long nodes = 1;
     if (nw == 1) {   // one in-span: its best candidate if the vertex weight is positive
@@ -744,12 +732,12 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
       bool solved = false;
       if (nw <= kSmallWindow) solved = stitch_small_window(sm, wb, E, nw, lane, &nodes);
       if (!solved) {
-        TW_SCOUNT(15, 1);
+        TW_COUNT(g_stitch_phase, 15, 1);
         nodes = stitch_mwis_large(wb, tb, E, nw, node_limit, lane);
       }
     }
     __syncwarp();
-    TW_SPHASE(7);                                // adjacency + MWIS
+    TW_PHASE(g_stitch_phase, phase_t0, 7);       // adjacency + MWIS
     if (nodes < 0) { rc = TW_ERR_MWIS_LIMIT; break; }
     if (nodes > max_nodes) max_nodes = nodes;
     int rank = -2;
@@ -769,7 +757,7 @@ __device__ __forceinline__ void stitch_unit(const tw_batch& b, const tw_params& 
     if (!tk_smem) __threadfence_block();
     __syncwarp();
     ws = we + 1;
-    TW_SPHASE(8);                                // window commit
+    TW_PHASE(g_stitch_phase, phase_t0, 8);       // window commit
   }
   if (lane == 0) {
     if (rc != TW_OK) atomicMin(err_flag, rc);
@@ -897,18 +885,6 @@ k_stitch_units(tw_batch b, const uint8_t* __restrict__ cut_all, tw_score_out spe
   }
   emit(unit_start, n);
 }
-
-#ifdef TW_PROFILE_PHASES
-extern "C" int tw_debug_stitch_phases(unsigned long long* out16, int reset) {
-  cudaError_t e = cudaMemcpyFromSymbol(out16, g_stitch_phase, sizeof(unsigned long long) * 16);
-  if (e != cudaSuccess) return -2;
-  if (reset) {
-    unsigned long long z[16] = {0};
-    cudaMemcpyToSymbol(g_stitch_phase, z, sizeof z);
-  }
-  return 0;
-}
-#endif
 
 #ifdef TW_STITCH_TIMELINE
 // out: [kTimelineCap][3] (start ns, end ns, smid) of every launched warp; zero where no warp ran
